@@ -23,9 +23,18 @@
  * score AND equal last character) straddling the beam cut or adjacent in the final order, and
  * equal probabilities straddling the cutoff_top_n cut, which the reference resolves through
  * libstdc++ introsort/introselect internals -- is resolved here deterministically (first in
- * trie DFS order wins) and reported through tie_flags so tests can mask those utterances.
+ * trie DFS order wins) and reported through tie_flags.
+ *
+ * At a beam-cut tie the reference keeps SOME r of the m comparator-equal prefixes that straddle
+ * the cut; which r is all its choice decides (the order of the kept prefixes changes no
+ * arithmetic: a node's per-frame sums have at most two terms and log_sum_exp is symmetric).
+ * ctc_oracle_decode_choices() takes one choice per such tie event -- an index into the r-subsets
+ * of the m members, 0 = the first r in DFS order, the default -- and reports every event, so a
+ * caller can enumerate every output the reference may produce.  Equal probabilities at the
+ * vocabulary cut keep the lowest indices (as the CUDA program does); they take no choice.
  */
 #include <float.h>
+#include <limits.h>
 #include <math.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -181,6 +190,40 @@ static void merge_sort_nodes(Node **a, Node **tmp, int n) {
   memcpy(a, tmp, sizeof(Node *) * n);
 }
 
+static int prefix_equiv(const Node *x, const Node *y) { return !prefix_compare(x, y) && !prefix_compare(y, x); }
+
+/* C(n, k), saturating at ULLONG_MAX */
+static unsigned long long binom(int n, int k) {
+  if (k < 0 || k > n) return 0;
+  if (k > n - k) k = n - k;
+  unsigned long long r = 1;
+  for (int i = 1; i <= k; ++i) { /* r = C(n-k+i-1, i-1) -> C(n-k+i, i), exact at every step */
+    unsigned __int128 t = (unsigned __int128)r * (unsigned)(n - k + i) / (unsigned)i;
+    if (t > ULLONG_MAX) return ULLONG_MAX;
+    r = (unsigned long long)t;
+  }
+  return r;
+}
+
+/* Reorder a[0..m) so that the r-subset of rank `choice` (lexicographic order of index sets: rank 0 = {0..r-1}) comes
+ * first, each part keeping its relative order.  Uses tmp[0..m) only: the kept part goes there, the dropped part is
+ * compacted in place (its write index never passes the read index). */
+static void keep_subset(Node **a, Node **tmp, int m, int r, unsigned long long choice) {
+  int k = r, nk = 0, nd = 0;
+  for (int i = 0; i < m; ++i) {
+    unsigned long long with_i = k > 0 ? binom(m - i - 1, k - 1) : 0;
+    if (k > 0 && choice < with_i) {
+      tmp[nk++] = a[i];
+      --k;
+    } else {
+      choice -= with_i;
+      a[nd++] = a[i];
+    }
+  }
+  memmove(a + nk, a, sizeof(Node *) * nd);
+  memcpy(a, tmp, sizeof(Node *) * nk);
+}
+
 /* ---- get_pruned_log_probs  (decoder_utils.cpp:10-45) ------------------------------------ */
 typedef struct {
   int idx;
@@ -235,6 +278,12 @@ typedef struct {
   /* what kind of ties straddled the beam cut (tools/tie_report.py): frames where the tied prefixes are -FLT_MAX
    * "junk" (SURVEY.md quirk Q6) / carry a finite score, and the first such frame */
   int tie_junk_frames, tie_finite_frames, tie_first_frame;
+  /* beam-cut tie control (ctc_oracle_decode_choices): the kept subset at the i-th tie event is tie_choice[i] (0 when
+   * i >= n_tie_choice); each event is logged as (frame, m, r, junk) into tie_events[4 * i] while i < max_tie_events */
+  const long long *tie_choice;
+  int n_tie_choice;
+  int *tie_events;
+  int max_tie_events, n_tie_events;
   /* scratch */
   ProbIdx *work;
   int *pr_idx;
@@ -315,12 +364,28 @@ void ctc_oracle_state_next(void *h, const float *probs, int num_time_steps) {
       }
       merge_sort_nodes(s->prefixes.v, s->tmp, s->prefixes.n);
       if (s->prefixes.n > s->beam_size) {
-        Node *a = s->prefixes.v[s->beam_size - 1], *b = s->prefixes.v[s->beam_size];
-        if (!prefix_compare(a, b) && !prefix_compare(b, a)) {
+        Node **v = s->prefixes.v;
+        const int K = s->beam_size;
+        if (prefix_equiv(v[K - 1], v[K])) {
           if (!(s->tie_flags & TIE_PRUNE)) s->tie_first_frame = s->abs_time_step;
           s->tie_flags |= TIE_PRUNE;
-          if (a->score <= -NUM_FLT_INF) s->tie_junk_frames++;
+          int junk = v[K]->score <= -NUM_FLT_INF;
+          if (junk) s->tie_junk_frames++;
           else s->tie_finite_frames++;
+          /* the tie event: the maximal run [lo, hi) of prefixes equivalent to v[K], in DFS order (stable sort) */
+          int lo = K - 1, hi = K + 1;
+          while (lo > 0 && prefix_equiv(v[lo - 1], v[K])) --lo;
+          while (hi < s->prefixes.n && prefix_equiv(v[hi], v[K])) ++hi;
+          int e = s->n_tie_events++;
+          if (e < s->max_tie_events) {
+            int *ev = s->tie_events + 4 * (size_t)e;
+            ev[0] = s->abs_time_step;
+            ev[1] = hi - lo;
+            ev[2] = K - lo;
+            ev[3] = junk;
+          }
+          long long choice = e < s->n_tie_choice ? s->tie_choice[e] : 0;
+          if (choice > 0) keep_subset(v + lo, s->tmp, hi - lo, K - lo, (unsigned long long)choice);
         }
       }
       for (int i = s->beam_size; i < s->prefixes.n; ++i) node_remove(s->prefixes.v[i]);
@@ -390,6 +455,27 @@ int ctc_oracle_decode_batch(const float *probs, const int *seq_lens, int B, int 
     ctc_oracle_state_free(st);
   }
   return 1;
+}
+
+/* One utterance (len frames of a [T, V] row block) with the beam-cut tie choices `choice[0..n_choice)` (further events:
+ * choice 0, i.e. exactly ctc_oracle_decode_batch's result).  Every tie event met is written as (frame, m, r, junk) to
+ * events[4 * i] for i < max_events; *n_events = how many were met.  Outputs as one utterance of the batch entry. */
+int ctc_oracle_decode_choices(const float *probs, int len, int T, int V, int beam_size, double cutoff_prob,
+                              int cutoff_top_n, int blank_id, int log_input, const long long *choice, int n_choice,
+                              int *events, int max_events, int *n_events, int *out_tokens, int *out_timesteps,
+                              float *out_scores, int *out_lens, int *tie_flags) {
+  if (len > T) len = T;
+  if (len < 0) len = 0;
+  OracleState *st = (OracleState *)ctc_oracle_state_new(V, beam_size, cutoff_prob, cutoff_top_n, blank_id, log_input);
+  st->tie_choice = choice;
+  st->n_tie_choice = n_choice;
+  st->tie_events = events;
+  st->max_tie_events = max_events;
+  ctc_oracle_state_next(st, probs, len);
+  int n = ctc_oracle_state_decode(st, T, out_tokens, out_timesteps, out_scores, out_lens, tie_flags);
+  *n_events = st->n_tie_events;
+  ctc_oracle_state_free(st);
+  return n;
 }
 
 /* libm probes used by the exhaustive device-vs-host float checks in tests/ (Appendix B of SURVEY.md) */

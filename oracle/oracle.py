@@ -11,8 +11,10 @@ instead of being left uninitialised), scores float32 [B, beam], lens int32 [B, b
 n_results int32 [B].
 """
 import ctypes
+import math
 import os
 import subprocess
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
@@ -46,6 +48,29 @@ def _prep(probs, seq_lens):
     return probs, seq_lens, B, T, V
 
 
+TIE_PRUNE, TIE_FINAL, TIE_VOCAB = 1, 2, 4   # tie_flags bits (ctc_oracle.c)
+
+
+def result_key(d, b=0):
+    """Hashable form of utterance b of a result dict: n_results and its rows (score bits, len, tokens, timesteps), rows
+    inside a run of equal (score bits, last token) sorted -- the reference's final sort may emit those in any order."""
+    n = int(d["n_results"][b])
+    rows = []
+    for p in range(n):
+        L = int(d["lens"][b, p])
+        rows.append((int(d["scores"][b, p:p + 1].view(np.int32)[0]), L, tuple(d["tokens"][b, p, :L].tolist()),
+                     tuple(d["timesteps"][b, p, :L].tolist())))
+    last = [r[2][-1] if r[1] else -1 for r in rows]
+    out, p = [], 0
+    while p < n:
+        q = p + 1
+        while q < n and rows[q][0] == rows[p][0] and last[q] == last[p]:
+            q += 1
+        out.extend(sorted(rows[p:q]))
+        p = q
+    return n, tuple(out)
+
+
 class CPort:
     """The plain-C restatement (no LM)."""
 
@@ -59,6 +84,11 @@ class CPort:
         L.ctc_oracle_decode_batch.argtypes = [_f32p, _i32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                               ctypes.c_double, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                               _i32p, _i32p, _f32p, _i32p, _i32p, _i32p]
+        L.ctc_oracle_decode_choices.restype = ctypes.c_int
+        L.ctc_oracle_decode_choices.argtypes = [_f32p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                                ctypes.c_double, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                                ctypes.c_void_p, ctypes.c_int, _i32p, ctypes.c_int, _i32p, _i32p,
+                                                _i32p, _f32p, _i32p, _i32p]
         L.ctc_oracle_state_new.restype = ctypes.c_void_p
         L.ctc_oracle_state_new.argtypes = [ctypes.c_int, ctypes.c_int, ctypes.c_double, ctypes.c_int, ctypes.c_int,
                                            ctypes.c_int]
@@ -81,6 +111,77 @@ class CPort:
                                          cutoff_top_n, blank_id, int(log_input), _p(tok, _i32p), _p(ts, _i32p),
                                          _p(sc, _f32p), _p(ln, _i32p), _p(nres, _i32p), _p(ties, _i32p))
         return dict(tokens=tok, timesteps=ts, scores=sc, lens=ln, n_results=nres, ties=ties)
+
+    def decode_choices(self, row, length, choices=(), beam=100, cutoff_prob=1.0, cutoff_top_n=40, blank_id=0,
+                       log_input=False):
+        """One utterance (row: [T, V]) with the beam-cut tie choices `choices` (see ctc_oracle_decode_choices; missing
+        ones are 0, which is decode()'s resolution).  Returns (result dict shaped like decode()'s for B = 1, events):
+        events is an int32 [n, 4] array of (frame, m, r, junk), one row per tie event met."""
+        row = np.ascontiguousarray(row, dtype=np.float32)
+        T, V = row.shape
+        tok, ts, sc, ln, _ = _alloc(1, beam, T)
+        ch = np.ascontiguousarray(choices, dtype=np.int64)
+        ev = np.zeros((max(T, 1), 4), np.int32)    # at most one tie event per frame
+        n_ev, tie = ctypes.c_int(0), ctypes.c_int(0)
+        n = self.lib.ctc_oracle_decode_choices(_p(row, _f32p), int(length), T, V, beam, cutoff_prob, cutoff_top_n,
+                                               blank_id, int(log_input), ch.ctypes.data, len(ch), _p(ev, _i32p),
+                                               ev.shape[0], ctypes.byref(n_ev), _p(tok, _i32p), _p(ts, _i32p),
+                                               _p(sc, _f32p), _p(ln, _i32p), ctypes.byref(tie))
+        out = dict(tokens=tok, timesteps=ts, scores=sc, lens=ln, n_results=np.array([n], np.int32),
+                   ties=np.array([tie.value], np.int32))
+        return out, ev[:n_ev.value]
+
+    def _enumerate(self, row, length, cap, kw):
+        """Depth-first walk over the choice vectors of one utterance: every leaf is one complete decode.  Returns (the
+        distinct outputs, the choice-0 decode first; unresolved; junk).  Unresolved: a tie among -FLT_MAX "junk"
+        prefixes (SURVEY.md quirk Q6; their groups are far too large to enumerate -- `junk` is then set) or more than
+        `cap` leaves."""
+        alts, seen, leaves = [], set(), 0
+        stack = [()]
+        while stack:
+            choices = stack.pop()
+            out, events = self.decode_choices(row, length, choices, **kw)
+            leaves += 1
+            if events[:, 3].any():
+                return alts or [out], True, True
+            key = result_key(out)
+            if key not in seen:
+                seen.add(key)
+                alts.append(out)
+            # branch at every event this run took the default for: events before len(choices) are fixed by `choices`
+            for j in range(len(events) - 1, len(choices) - 1, -1):
+                k = math.comb(int(events[j, 1]), int(events[j, 2]))
+                if leaves + len(stack) + k - 1 > cap:
+                    return alts, True, False
+                pad = choices + (0,) * (j - len(choices))
+                stack.extend(pad + (c,) for c in range(k - 1, 0, -1))
+        return alts, False, False
+
+    def decode_alternatives(self, probs, seq_lens=None, cap=64, beam=100, cutoff_prob=1.0, cutoff_top_n=40,
+                            blank_id=0, log_input=False, threads=None):
+        """decode(), plus every output the reference may produce where it is unspecified.  At a beam-cut tie
+        (TIE_PRUNE) the reference keeps some r of the m comparator-equal prefixes straddling the cut; for each
+        TIE_PRUNE-flagged utterance every combination of such choices is decoded.  Adds to decode()'s dict:
+          alternatives[b]  list of distinct B = 1 result dicts (alternatives[b][0] is decode()'s own row);
+          unresolved[b]    bool: junk ties or more than `cap` choice vectors -- the list is then incomplete;
+          junk_ties[b]     bool: unresolved because a tie among -FLT_MAX junk prefixes was met.
+        Distinct means: tokens, timesteps, score bits, lens and n_results differ after rows of equal (score, last
+        token) -- which the reference's final sort may emit in either order (TIE_FINAL) -- are put in canonical order.
+        Flagged utterances are enumerated on `threads` threads (the C calls release the GIL)."""
+        kw = dict(beam=beam, cutoff_prob=cutoff_prob, cutoff_top_n=cutoff_top_n, blank_id=blank_id, log_input=log_input)
+        base = self.decode(probs, seq_lens, **kw)
+        probs, seq_lens, B, T, V = _prep(probs, seq_lens)
+        alts = [[{k: v[b:b + 1] for k, v in base.items()}] for b in range(B)]
+        unresolved, junk = np.zeros((B,), bool), np.zeros((B,), bool)
+        todo = [b for b in range(B) if base["ties"][b] & TIE_PRUNE]
+        if todo:
+            with ThreadPoolExecutor(threads or len(os.sched_getaffinity(0))) as ex:
+                for b, res in zip(todo, ex.map(lambda b: self._enumerate(probs[b], seq_lens[b], cap, kw), todo)):
+                    alts[b], unresolved[b], junk[b] = res
+        base["alternatives"] = alts
+        base["unresolved"] = unresolved
+        base["junk_ties"] = junk
+        return base
 
     # --- streaming (mirrors DecoderState next()/decode()) ---
     def state_new(self, V, beam, cutoff_prob=1.0, cutoff_top_n=40, blank_id=0, log_input=False):

@@ -56,6 +56,20 @@ REFERENCE_BUILD_CASES = {
     "flat_T100_V29_beam50": (4, 100, 29, 15, True, dict(beam=50)),
 }
 
+# tests/test_oracle.py::test_enumerator_admits_reference_build_output: quantised rows (tests/tie_inputs.py), full of
+# comparator-equal prefixes at the beam cut -- (B, T, V, seed, levels, decoder arguments)
+REFERENCE_BUILD_TIE_CASES = {
+    "quant_T24_V5_beam3": (16, 24, 5, 35, (1.0, 2.0, 4.0), dict(beam=3, blank_id=4)),
+    "quant_T24_V4_beam8_cp09": (16, 24, 4, 84, (1.0, 2.0, 3.0), dict(beam=8, cutoff_prob=0.9)),
+}
+
+
+def emit_tie_cases():
+    from tests.tie_inputs import quantised_probs
+    for name, (B, T, V, seed, levels, kw) in REFERENCE_BUILD_TIE_CASES.items():
+        emit(os.path.join("reference_build", name), quantised_probs(B, T, V, seed, levels), **kw)
+
+
 L29 = ["_"] + [chr(ord("a") + i) for i in range(26)] + [" ", "'"]
 TINY_LM = os.path.join(ROOT, "tests", "data", "tiny_lm.arpa")
 
@@ -105,3 +119,4 @@ if __name__ == "__main__":
     for name, (B, T, V, seed, flat, kw) in REFERENCE_BUILD_CASES.items():
         probs = (flat_probs(B, T, V, seed) if flat else ctc_like_probs(B, T, V, seed)).numpy()
         emit(os.path.join("reference_build", name), probs, **kw)
+    emit_tie_cases()

@@ -2,17 +2,28 @@
 oracle.oracle / tests.emul / the CUDA path), honouring the reference's "unspecified" cases.
 
 Integer outputs (tokens, timesteps, lens, n_results) must be identical on [:len]; scores must be identical
-as float32 bit patterns (stronger than the 1e-4 the spec asks for).  Utterances whose tie flags are set
-by either side are handled as follows: a tie at a CUT (beam prune, vocabulary prune) can change which of two equally
-scored prefixes lives on, so for those utterances only what cannot depend on that choice is compared (number of
-results, multiset of score bits, the best beam when its score is unique) and they are counted as "skipped"; a tie only in the FINAL order (two result rows with the same
-score and the same last character, which std::sort may emit in either order) is compared row-set-wise inside
-each tied group -- everything else about the utterance must still match exactly.  Beams with score == FLT_MAX are -FLT_MAX "junk" prefixes
-(SURVEY.md quirk Q6) whose relative order is a tie by construction.
+as float32 bit patterns (stronger than the 1e-4 the spec asks for).  Beams with score == FLT_MAX are -FLT_MAX "junk"
+prefixes (SURVEY.md quirk Q6) whose relative order is a tie by construction: only their pattern is compared.  A tie
+in the FINAL order (two result rows with the same score and the same last character, which std::sort may emit in
+either order) is compared row-set-wise inside each tied group -- everything else about the utterance must still match.
+
+A tie at a CUT (the beam prune, TIE_PRUNE; the vocabulary prune, TIE_VOCAB) lets the reference keep either of two
+equally ranked prefixes.  How compare() treats such an utterance depends on the reference it is given:
+
+* ``ref`` from ``CPort.decode_alternatives`` (the C oracle, which can be steered through its beam-cut ties): every
+  output the reference may produce at those ties is known, and ``got`` must equal one of them under the rules above.
+  TIE_VOCAB is compared exactly against the oracle's fixed resolution (lowest indices, which the CUDA program keeps
+  too); the reference's unstable std::sort may keep other indices there, which is not enumerated.  Only utterances the
+  enumerator marks "unresolved" fall back to comparing n_results -- ties among -FLT_MAX junk prefixes, whose groups are
+  far too large to enumerate, and utterances whose choice vectors exceed ``cap`` (tie frames chaining on inputs built
+  to tie); compare() returns them as its second count.
+* any other ``ref`` (a plain decode, the unmodified reference build, the golden fixtures): utterances whose tie flags
+  show a cut tie on either side are "skipped" -- only n_results is asserted.
 """
 import numpy as np
 
 FLT_MAX = np.float32(3.4028235e38)
+_KEYS = ("tokens", "timesteps", "scores", "lens", "n_results", "ties")
 
 
 def _canonicalise(d, b):
@@ -62,10 +73,72 @@ def _align_permuted_runs(ref, got, b):
         p = q
 
 
+def _utterance(d, b):
+    return {k: d[k][b:b + 1] for k in _KEYS if k in d}
+
+
+def _compare_alternatives(ref, got, name):
+    checked, unresolved = 0, 0
+    for b in range(ref["lens"].shape[0]):
+        if ref["unresolved"][b]:
+            unresolved += 1
+            assert int(got["n_results"][b]) == int(ref["n_results"][b]), f"{name} utt {b} (unresolved): n_results differ"
+            continue
+        one = _utterance(got, b)
+        got_final = int(one["ties"][0]) & 2 if "ties" in one else 0
+        alts = ref["alternatives"][b]
+        first_error = None
+        for alt in alts:
+            try:
+                _compare_exact(alt, one, 0, (int(alt["ties"][0]) & 2) | got_final, name)
+                break
+            except AssertionError as e:
+                first_error = first_error or e
+        else:
+            raise AssertionError(f"{name} utt {b}: equals none of the {len(alts)} outputs the reference may produce; "
+                                 f"against the first: {first_error}")
+        checked += 1
+    return checked, unresolved
+
+
+def _compare_exact(ref, got, b, final_tie, name):
+    if final_tie:  # FLAG_TIE_FINAL: canonical order inside groups of equal (score, last char)
+        ref = dict(ref)
+        got = dict(got)
+        for d in (ref, got):
+            for key in ("tokens", "timesteps", "scores", "lens"):
+                d[key] = d[key].copy()
+            _canonicalise(d, b)
+        # With a scorer the tied rows cannot be told from the REPORTED scores (the order is by the raw prefix score,
+        # the reported score is the LM-corrected one, reference :187-208): every maximal run of rows that differ
+        # must then hold the same rows on both sides, in any order.
+        _align_permuted_runs(ref, got, b)
+    n = int(ref["n_results"][b])
+    assert int(got["n_results"][b]) == n, f"{name} utt {b}: n_results {got['n_results'][b]} != {n}"
+    rs, gs = ref["scores"][b, :n], got["scores"][b, :n]
+    junk = rs == FLT_MAX
+    assert np.array_equal(junk, gs == FLT_MAX), f"{name} utt {b}: junk beam pattern differs"
+    ok = ~junk
+    assert np.array_equal(rs[ok].view(np.int32), gs[ok].view(np.int32)), \
+        f"{name} utt {b}: scores differ\n{rs[ok][:8]}\n{gs[ok][:8]}"
+    assert np.array_equal(ref["lens"][b, :n][ok], got["lens"][b, :n][ok]), f"{name} utt {b}: lens differ"
+    for p in range(n):
+        if junk[p]:
+            continue
+        L = int(ref["lens"][b, p])
+        assert np.array_equal(ref["tokens"][b, p, :L], got["tokens"][b, p, :L]), \
+            f"{name} utt {b} beam {p}: tokens differ\n{ref['tokens'][b, p, :L]}\n{got['tokens'][b, p, :L]}"
+        assert np.array_equal(ref["timesteps"][b, p, :L], got["timesteps"][b, p, :L]), \
+            f"{name} utt {b} beam {p}: timesteps differ\n{ref['timesteps'][b, p, :L]}\n{got['timesteps'][b, p, :L]}"
+
+
 def compare(ref, got, ref_ties=None, name=""):
-    B = ref["lens"].shape[0]
+    """Asserts parity utterance by utterance; returns (checked, skipped).  With a ``ref`` from
+    CPort.decode_alternatives the second count is the number of unresolved utterances (see the module docstring)."""
+    if "alternatives" in ref:
+        return _compare_alternatives(ref, got, name)
     skipped, checked = 0, 0
-    for b in range(B):
+    for b in range(ref["lens"].shape[0]):
         tie = 0
         if ref_ties is not None:
             tie |= int(ref_ties[b])
@@ -80,35 +153,8 @@ def compare(ref, got, ref_ties=None, name=""):
             skipped += 1
             assert int(got["n_results"][b]) == int(ref["n_results"][b]), f"{name} utt {b} (tie-flagged): n_results differ"
             continue
-        if tie & 2:  # FLAG_TIE_FINAL only: canonical order inside groups of equal (score, last char)
-            ref = dict(ref)
-            got = dict(got)
-            for d in (ref, got):
-                for key in ("tokens", "timesteps", "scores", "lens"):
-                    d[key] = d[key].copy()
-                _canonicalise(d, b)
-            # With a scorer the tied rows cannot be told from the REPORTED scores (the order is by the raw prefix score,
-            # the reported score is the LM-corrected one, reference :187-208): every maximal run of rows that differ
-            # must then hold the same rows on both sides, in any order.
-            _align_permuted_runs(ref, got, b)
+        _compare_exact(ref, got, b, tie & 2, name)
         checked += 1
-        n = int(ref["n_results"][b])
-        assert int(got["n_results"][b]) == n, f"{name} utt {b}: n_results {got['n_results'][b]} != {n}"
-        rs, gs = ref["scores"][b, :n], got["scores"][b, :n]
-        junk = rs == FLT_MAX
-        assert np.array_equal(junk, gs == FLT_MAX), f"{name} utt {b}: junk beam pattern differs"
-        ok = ~junk
-        assert np.array_equal(rs[ok].view(np.int32), gs[ok].view(np.int32)), \
-            f"{name} utt {b}: scores differ\n{rs[ok][:8]}\n{gs[ok][:8]}"
-        assert np.array_equal(ref["lens"][b, :n][ok], got["lens"][b, :n][ok]), f"{name} utt {b}: lens differ"
-        for p in range(n):
-            if junk[p]:
-                continue
-            L = int(ref["lens"][b, p])
-            assert np.array_equal(ref["tokens"][b, p, :L], got["tokens"][b, p, :L]), \
-                f"{name} utt {b} beam {p}: tokens differ\n{ref['tokens'][b, p, :L]}\n{got['tokens'][b, p, :L]}"
-            assert np.array_equal(ref["timesteps"][b, p, :L], got["timesteps"][b, p, :L]), \
-                f"{name} utt {b} beam {p}: timesteps differ\n{ref['timesteps'][b, p, :L]}\n{got['timesteps'][b, p, :L]}"
     return checked, skipped
 
 

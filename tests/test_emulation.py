@@ -6,18 +6,21 @@ import numpy as np
 import pytest
 
 from ctcdecode_b200.synth import ctc_like_probs, flat_probs
-from tests import emul, golden_util
+from tests import emul, golden_util, tie_inputs
 from tests.parity import compare
 
 
 def _check(cport, probs, seq_lens=None, nt=0, chunk=0, **kw):
-    ref = cport.decode(probs, seq_lens, **kw)
+    """Emulation == one of the outputs the reference may produce, on every utterance; only utterances with ties among
+    -FLT_MAX junk prefixes may stay unresolved.  Returns (checked, unresolved)."""
+    ref = cport.decode_alternatives(probs, seq_lens, **kw)
     got = emul.decode(probs, seq_lens, nt=nt, chunk=chunk, **kw)
-    checked, skipped = compare(ref, got, ref["ties"], str(kw))
+    checked, unresolved = compare(ref, got, ref["ties"], str(kw))
+    assert np.array_equal(ref["unresolved"], ref["junk_ties"]), "enumeration exceeded its cap on a finite tie"
     # the emulation must flag exactly the utterances the oracle flags
     assert np.array_equal(ref["ties"] != 0, (got["ties"] & 7) != 0)
     assert not (got["ties"] & 256).any()
-    return checked, skipped
+    return checked, unresolved
 
 
 @pytest.mark.parametrize("name", golden_util.names())
@@ -86,6 +89,93 @@ def test_emulation_streaming_state_roundtrip(cport, chunk):
     _check(cport, probs, seq_lens=np.array([90, 45, 3], np.int32), chunk=chunk, beam=24)
     p2 = ctc_like_probs(1, 64, 100, seed=23).numpy()
     _check(cport, p2, chunk=chunk, beam=12, cutoff_top_n=15)
+
+
+@pytest.mark.parametrize("cfg", [
+    dict(V=3, beam=5, temp=2.0),
+    dict(V=4, beam=8, temp=1.0),
+    dict(V=5, beam=10, temp=1.0, blank_id=4, cutoff_prob=0.9),
+    dict(V=6, beam=16, temp=0.5, blank_id=5),
+    dict(V=6, beam=12, temp=1.0, cutoff_top_n=4),
+])
+def test_emulation_flat_small_vocabulary_ties(cport, cfg):
+    """Flat rows over 3-6 labels: tie-flagged utterances are compared against every output the reference may
+    produce, not skipped."""
+    cfg = dict(cfg)
+    V, temp = cfg.pop("V"), cfg.pop("temp")
+    probs = flat_probs(8, 150, V, seed=V, temp=temp).numpy()
+    checked, unresolved = _check(cport, probs, **cfg)
+    assert checked + unresolved == 8
+
+
+@pytest.mark.parametrize("cfg", [
+    dict(V=3, beam=5, levels=(1.0, 2.0)),
+    dict(V=4, beam=8),
+    dict(V=5, beam=3, blank_id=4),
+    dict(V=5, beam=6, blank_id=4, cutoff_prob=0.9, levels=(1.0, 2.0, 3.0)),
+    dict(V=6, beam=10, levels=(1.0, 2.0, 3.0, 5.0)),
+    dict(V=6, beam=6, cutoff_top_n=4, levels=(1.0, 2.0, 3.0, 5.0, 7.0)),
+    dict(V=6, beam=10, log_input=True, levels=(1.0, 2.0, 3.0, 5.0)),
+], ids=["V3", "V4", "V5_beam3", "V5_cp", "V6", "V6_top4", "V6_log"])
+@pytest.mark.parametrize("nt", [0, 128])
+def test_emulation_quantised_rows_prune_ties(cport, cfg, nt):
+    """Probabilities quantised to a few values: equal scores at the beam cut in many frames (TIE_PRUNE).  Every
+    utterance must equal one of the outputs the reference may produce.  A few utterances chain so many tie frames that
+    their choice vectors exceed the enumeration cap; they count as unresolved and are bounded here."""
+    cfg = dict(cfg)
+    V, levels = cfg.pop("V"), cfg.pop("levels", (1.0, 2.0, 4.0))
+    probs = tie_inputs.quantised_probs(16, 24, V, seed=V + 10 * cfg["beam"], levels=levels)
+    if cfg.get("log_input"):
+        probs = np.log(probs)
+    ref = cport.decode_alternatives(probs, cap=256, **cfg)
+    assert (ref["ties"] & 1).sum() >= 6                    # the input does what it is for
+    got = emul.decode(probs, nt=nt, **cfg)
+    checked, unresolved = compare(ref, got, ref["ties"], str(cfg))
+    assert checked + unresolved == 16 and checked >= 13
+    assert np.array_equal(ref["ties"] != 0, (got["ties"] & 7) != 0)
+
+
+def test_emulation_quantised_rows_need_alternatives(cport):
+    """The quantised inputs above are not vacuous: on them the CTA program keeps a different (equally ranked) prefix
+    than the oracle's default resolution in some utterances, which the old skip-and-count rule never looked at."""
+    n = 0
+    for V, beam, blank in ((4, 8, 0), (5, 3, 4), (6, 10, 0)):
+        probs = tie_inputs.quantised_probs(16, 24, V, seed=V + 10 * beam)
+        ref = cport.decode_alternatives(probs, cap=256, beam=beam, blank_id=blank)
+        got = emul.decode(probs, beam=beam, blank_id=blank)
+        compare(ref, got, ref["ties"], "quantised V%d" % V)
+        n += tie_inputs.resolved_by_alternative(ref, got)
+    assert n > 0
+
+
+def test_emulation_config4_row_with_a_finite_prune_tie(cport):
+    """A config-4 utterance (T = 2000, V = 256, beam 200, cutoff_prob 0.99) with one finite-score tie at the beam cut
+    (frame 1632: two prefixes, one kept).  The oracle decodes it twice; the CTA program must equal one of the two."""
+    probs = ctc_like_probs(2, 2000, 256, seed=0).numpy()[1:2]
+    ref = cport.decode_alternatives(probs, beam=200, cutoff_prob=0.99)
+    assert ref["ties"][0] & 1 and not ref["unresolved"][0]
+    got = emul.decode(probs, beam=200, cutoff_prob=0.99)
+    assert compare(ref, got, ref["ties"], "config 4, utterance 1") == (1, 0)
+
+
+@pytest.mark.parametrize("path", list(tie_inputs.PRUNE_PATHS))
+@pytest.mark.parametrize("kind", tie_inputs.DEGENERATE)
+def test_emulation_degenerate_values(cport, kind, path):
+    """Exact zeros, subnormal probabilities, probabilities above 1, one-hot blank frames, -inf / -FLT_MAX / -1e30 /
+    positive log-probabilities and blank at -inf for whole stretches, through every vocabulary-cut configuration.
+    Unresolved utterances (n_results only) occur in three cells: -FLT_MAX junk ties with cutoff_prob (above_one: 1 of
+    6, log_extremes: 3 of 6), and, in log_extremes with the top-40 cut of 256 labels, 2 of 6 whose finite ties chain
+    past the enumeration cap (-1e30 absorbs any score it is added to).  Every cell checks at least 3 of its 6
+    utterances exactly, and only log_extremes may leave a finite tie unresolved."""
+    V, kw = tie_inputs.PRUNE_PATHS[path]
+    probs, log_input = tie_inputs.degenerate_probs(kind, 6, 40, V, seed=V)
+    ref = cport.decode_alternatives(probs, cap=256, log_input=log_input, **kw)
+    got = emul.decode(probs, log_input=log_input, **kw)
+    checked, unresolved = compare(ref, got, ref["ties"], "%s %s" % (kind, path))
+    assert checked + unresolved == 6 and checked >= 3
+    assert (ref["unresolved"] & ~ref["junk_ties"]).sum() == 0 or kind == "log_extremes"
+    assert np.array_equal(ref["ties"] != 0, (got["ties"] & 7) != 0)
+    assert not (got["ties"] & 256).any()
 
 
 def test_emulation_uniform_input_massive_ties(cport):

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from ctcdecode_b200.synth import ctc_like_probs, flat_probs
-from tests import golden_util
+from tests import emul, golden_util, tie_inputs
 from tests.parity import compare
 
 pytestmark = pytest.mark.gpu
@@ -72,7 +72,7 @@ def test_cuda_matches_oracle(cport, cfg):
         probs = ctc_like_probs(B, T, V, seed, peak=peak, blank_id=cfg.get("blank_id", 0), log=log).numpy()
     if log:
         cfg["log_input"] = True
-    ref = cport.decode(probs, **cfg)
+    ref = cport.decode_alternatives(probs, **cfg)
     got = _run(probs, **cfg)
     compare(ref, got, ref["ties"], str(cfg))
     assert np.array_equal(ref["ties"] != 0, (got["ties"] & 7) != 0)
@@ -82,7 +82,7 @@ def test_cuda_matches_oracle(cport, cfg):
 def test_ragged_empty_and_host_path(cport):
     probs = ctc_like_probs(8, 120, 29, seed=21).numpy()
     sl = np.array([120, 0, 1, 7, 64, 119, 200, 33], np.int32)
-    ref = cport.decode(probs, sl, beam=32)
+    ref = cport.decode_alternatives(probs, sl, beam=32)
     for on_device in (True, False):
         got = _run(probs, sl, on_device=on_device, beam=32)
         compare(ref, got, ref["ties"], "ragged")
@@ -136,7 +136,7 @@ def test_online_decoder_matches_reference_tests_and_offline(cport):
     assert res.shape[2] >= int(lens.max())
     # chunked == offline on a seeded utterance batch, all beams
     p = ctc_like_probs(3, 160, 29, seed=31)
-    ref = cport.decode(p.numpy(), beam=24)
+    ref = cport.decode_alternatives(p.numpy(), beam=24)
     dec3 = ctcdecode.OnlineCTCBeamDecoder([str(i) for i in range(29)], beam_width=24)
     states = [ctcdecode.DecoderState(dec3) for _ in range(3)]
     for a, b in [(0, 50), (50, 51), (51, 130)]:
@@ -157,9 +157,9 @@ def test_full_size_config2_properties(cport):
     out, scores, ts, lens = dec.decode(d)
     flags, nres = dec.last_flags.clone(), dec.last_n_results.clone()
     assert int((flags & 256).sum()) == 0 and bool((nres == K).all())
-    # parity skips utterances with a comparator-equal pair at the beam cut (reference: unspecified); on this batch that
-    # is 7 of 256, each with one such frame, and 6 of the 7 still equal the reference build (tools/tie_report.py,
-    # DESIGN.md section 8).  Ties that only permute equal-key rows of the final order (10 more) are compared.
+    # utterances with a comparator-equal pair at the beam cut (reference: unspecified) are 7 of 256 on this batch, each
+    # with one such frame (tools/tie_report.py, DESIGN.md section 8); against the oracle they are compared with every
+    # output the reference may produce, but bench.py's comparison with the reference build skips them.
     assert int(((flags & 5) != 0).sum()) <= 12
     # determinism
     out2, scores2, ts2, lens2 = dec.decode(d)
@@ -178,12 +178,16 @@ def test_full_size_config2_properties(cport):
     assert bool(((tok >= 1) & (tok < V)).all())
     tsv = torch.where(valid, ts, 0)
     assert bool(((tsv >= 0) & (tsv < T)).all())
-    # exact slice against the oracle
-    sl = [0, 77, 255]
-    ref = cport.decode(probs[sl].numpy(), beam=K)
+    # exact slice against the oracle: three fixed utterances and the first three with a tie at a cut
+    tied = torch.nonzero((flags & 5) != 0).flatten().tolist()
+    assert len(tied) >= 3
+    sl = sorted(set([0, 77, 255] + tied[:3]))
+    ref = cport.decode_alternatives(probs[sl].numpy(), beam=K)
     got = dict(tokens=out[sl].cpu().numpy(), timesteps=ts[sl].cpu().numpy(), scores=scores[sl].cpu().numpy(),
                lens=lens[sl].cpu().numpy(), n_results=nres[sl].cpu().numpy(), ties=flags[sl].cpu().numpy())
-    compare(ref, got, ref["ties"], "config2 slice")
+    checked, unresolved = compare(ref, got, ref["ties"], "config2 slice")
+    assert (checked, unresolved) == (len(sl), 0)
+    print("config2 slice: %d prune/vocab-tie utterances checked" % int(((ref["ties"] & 5) != 0).sum()))
 
 
 def test_full_size_config4_slice(cport):
@@ -194,11 +198,13 @@ def test_full_size_config4_slice(cport):
     out, scores, ts, lens = dec.decode(probs.cuda())
     assert int((dec.last_flags & 256).sum()) == 0
     sl = [3, 12]
-    ref = cport.decode(probs[sl].numpy(), beam=200, cutoff_prob=0.99)
+    ref = cport.decode_alternatives(probs[sl].numpy(), beam=200, cutoff_prob=0.99)
     got = dict(tokens=out[sl].cpu().numpy(), timesteps=ts[sl].cpu().numpy(), scores=scores[sl].cpu().numpy(),
                lens=lens[sl].cpu().numpy(), n_results=dec.last_n_results[sl].cpu().numpy(),
                ties=dec.last_flags[sl].cpu().numpy())
-    compare(ref, got, ref["ties"], "config4 slice")
+    checked, unresolved = compare(ref, got, ref["ties"], "config4 slice")
+    assert (checked, unresolved) == (2, 0)
+    print("config4 slice: %d prune/vocab-tie utterances checked" % int(((ref["ties"] & 5) != 0).sum()))
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float16, torch.bfloat16], ids=["f32", "f16", "bf16"])
@@ -226,7 +232,7 @@ def test_decode_logits_fused_log_softmax(cport, dtype, cfg):
     lsm_cpu = lsm.cpu()
     for b, n in enumerate(seq_lens.tolist()):
         lsm_cpu[b, n:] = 0.0   # frames beyond seq_len are never read (nor written)
-    want = cport.decode(lsm_cpu.numpy(), seq_lens.numpy(), beam=beam, log_input=True, **cfg)
+    want = cport.decode_alternatives(lsm_cpu.numpy(), seq_lens.numpy(), beam=beam, log_input=True, **cfg)
     got = dict(tokens=out.numpy(), timesteps=ts.numpy(), scores=scores.numpy(), lens=lens.numpy(),
                n_results=dec.last_n_results.numpy(), ties=dec.last_flags.numpy())
     compare(want, got, want["ties"], "logits %s %s" % (dtype, cfg))
@@ -296,7 +302,7 @@ def test_large_batches_match_oracle(cport, cfg, on_device):
     rng = np.random.RandomState(seed)
     seq_lens = rng.randint(0, T + 1, size=B).astype(np.int32)
     seq_lens[:3] = [T, 0, 1]
-    ref = cport.decode(probs, seq_lens=seq_lens, **cfg)
+    ref = cport.decode_alternatives(probs, seq_lens=seq_lens, **cfg)
     got = _run(probs, seq_lens, on_device=on_device, **cfg)
     compare(ref, got, ref["ties"], str(cfg))
     assert np.array_equal(ref["ties"] != 0, (got["ties"] & 7) != 0)
@@ -326,7 +332,7 @@ def test_list_overflow_rewalk(cport, monkeypatch, seg):
                       (ctc_like_probs(2, 200, 256, seed=51).numpy(), dict(beam=200, cutoff_prob=0.99)),
                       (ctc_like_probs(2, 80, 64, seed=52).numpy(), dict(beam=32, cutoff_top_n=12)),
                       (flat_probs(2, 200, 4, seed=5, temp=1.0).numpy(), dict(beam=16))):
-        ref = cport.decode(probs, **kw)
+        ref = cport.decode_alternatives(probs, **kw)
         got = _run(probs, **kw)
         compare(ref, got, ref["ties"], "seg %d %s" % (seg, kw))
         assert not (got["ties"] & 256).any()
@@ -341,7 +347,109 @@ def test_checked_bound_failure_is_redone(cport, monkeypatch, bias):
                       (flat_probs(2, 120, 12, seed=6, temp=1.0).numpy(), dict(beam=16, cutoff_top_n=5)),
                       (ctc_like_probs(4, 300, 29, seed=53).numpy(), dict(beam=100)),   # index-order kernel
                       (flat_probs(2, 150, 6, seed=7, temp=1.5).numpy(), dict(beam=24))):
-        ref = cport.decode(probs, **kw)
+        ref = cport.decode_alternatives(probs, **kw)
         got = _run(probs, **kw)
         compare(ref, got, ref["ties"], "bias %s %s" % (bias, kw))
         assert not (got["ties"] & 256).any()
+
+
+FLAG_ERR_ARENA = 256
+
+
+def _tie_prone_batches():
+    q = tie_inputs.quantised_probs
+    return [(q(16, 24, 4, 2), dict(beam=8)),
+            (q(16, 24, 5, 3), dict(beam=3, blank_id=4)),
+            (q(16, 24, 6, 5, (1.0, 2.0, 3.0, 5.0)), dict(beam=10, cutoff_top_n=4)),
+            (q(8, 60, 5, 9, (1.0, 2.0, 3.0)), dict(beam=40, cutoff_prob=0.9)),
+            (np.log(q(8, 40, 6, 11)), dict(beam=12, log_input=True)),
+            (flat_probs(8, 200, 4, seed=5, temp=1.0).numpy(), dict(beam=16)),
+            (flat_probs(8, 200, 6, seed=8, temp=0.5).numpy(), dict(beam=16, blank_id=5)),
+            (tie_inputs.degenerate_probs("onehot_blank", 4, 60, 64, seed=3)[0], dict(beam=16, cutoff_top_n=12))]
+
+
+@pytest.mark.parametrize("nt", [128, 256])
+def test_device_equals_emulation_on_tie_prone_batches(monkeypatch, nt):
+    """The device and the CPU emulation run one deterministic program, ties included: with the block size forced on
+    both sides, every row of every utterance and every flag bit must be identical -- no tie exemption, no reordering
+    of equal-key rows.  (The tie list of the general back half is filled through atomicAdd; its order must never reach
+    a decision.)"""
+    monkeypatch.setenv("CTCDEC_NT", str(nt))
+    flagged = 0
+    for probs, kw in _tie_prone_batches():
+        got = _run(probs, **kw)
+        want = emul.decode(probs, nt=nt, **kw)
+        assert np.array_equal(got["ties"], want["ties"]), (kw, got["ties"], want["ties"])
+        flagged += int(((want["ties"] & 5) != 0).sum())
+        a, b = dict(got), dict(want)
+        a["ties"] = b["ties"] = np.zeros_like(a["ties"])
+        checked, _ = compare(b, a, None, "device vs emulation, nt %d, %s" % (nt, kw))
+        assert checked == probs.shape[0]
+    assert flagged >= 40
+    print("device == emulation (nt %d): %d prune/vocab-tie utterances compared row for row" % (nt, flagged))
+
+
+@pytest.mark.parametrize("path", list(tie_inputs.PRUNE_PATHS))
+@pytest.mark.parametrize("kind", tie_inputs.DEGENERATE)
+def test_degenerate_values_through_every_prune_path(cport, kind, path):
+    """Exact zeros, subnormal probabilities, probabilities above 1, one-hot blank frames, -inf / -FLT_MAX / -1e30 /
+    positive log-probabilities and blank at -inf for whole stretches, through each path of the device's vocabulary cut
+    (index order with V <= 32 and the wide-row loop, partial top_select, top_select with > 64 keys equal to the cut,
+    the full bitonic sort, cutoff_prob): equal to a permitted output of the oracle, no error flag.  As in
+    tests/test_emulation.py::test_emulation_degenerate_values, every cell checks at least 3 of its 6 utterances
+    exactly, and only log_extremes may leave a finite tie unresolved."""
+    V, kw = tie_inputs.PRUNE_PATHS[path]
+    probs, log_input = tie_inputs.degenerate_probs(kind, 6, 40, V, seed=V)
+    ref = cport.decode_alternatives(probs, cap=256, log_input=log_input, **kw)
+    for on_device in (True, False):
+        got = _run(probs, on_device=on_device, log_input=log_input, **kw)
+        checked, unresolved = compare(ref, got, ref["ties"], "%s %s" % (kind, path))
+        assert checked + unresolved == 6 and checked >= 3
+        assert (ref["unresolved"] & ~ref["junk_ties"]).sum() == 0 or kind == "log_extremes"
+        assert np.array_equal(ref["ties"] != 0, (got["ties"] & 7) != 0)
+        assert not (got["ties"] & FLAG_ERR_ARENA).any()
+
+
+@pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16], ids=["f16", "bf16"])
+@pytest.mark.parametrize("cfg", [dict(V=29, beam=16), dict(V=64, beam=16, cutoff_top_n=12),
+                                 dict(V=256, beam=16, cutoff_top_n=40), dict(V=64, beam=16, cutoff_prob=0.99)],
+                         ids=["index", "top12", "top40_v256", "cp99"])
+def test_decode_logits_with_inf_and_fp16_extremes(cport, dtype, cfg):
+    """Half-precision logits with -inf entries and the fp16 extremes (+-65504): the fused log-softmax agrees with a
+    float64 log-softmax to 4e-6, the rows it returns decode through the oracle to the same result, no error flag."""
+    from ctcdecode_b200 import CTCBeamDecoder
+    cfg = dict(cfg)
+    V, beam = cfg.pop("V"), cfg.pop("beam")
+    x = ctc_like_probs(3, 80, V, seed=81, raw_logits=True)
+    g = torch.Generator().manual_seed(82)
+    u = torch.rand(x.shape, generator=g)
+    x = torch.where(u < 0.15, torch.tensor(float("-inf")), x)
+    x = torch.where((u >= 0.15) & (u < 0.17), torch.tensor(-65504.0), x)
+    x[:, ::7, 1] = 65504.0                              # a row's maximum at the fp16 limit
+    x[:, :, 0] = torch.where(u[:, :, 0] < 0.5, x[:, :, 0], torch.tensor(0.0))   # never a row of only -inf
+    x = x.to(dtype).cuda()
+    seq_lens = torch.tensor([80, 51, 0], dtype=torch.int32)
+    dec = CTCBeamDecoder([str(i) for i in range(V)], beam_width=beam, **cfg)
+    out, scores, ts, lens, lsm = dec.decode_logits(x, seq_lens, return_log_probs=True)
+    want_lsm = torch.log_softmax(x.double(), dim=-1).to(lsm.device)
+    for b, n in enumerate(seq_lens.tolist()):
+        assert torch.equal(torch.isneginf(lsm[b, :n]), torch.isneginf(want_lsm[b, :n]))
+        fin = torch.isfinite(want_lsm[b, :n])
+        assert bool(torch.isfinite(lsm[b, :n][fin]).all())
+        # 4e-6 absolute as for ordinary logits, or two float32 ulps of the exact value where those are coarser: values
+        # near -65504 (against an ordinary maximum) or -131008 (against a +65504 one) are spaced 2^-8 / 2^-7 apart in
+        # float32.  Below |x| = 32 two ulps are under 4e-6, so ordinary values keep the 4e-6 bound.
+        w = want_lsm[b, :n][fin]
+        w32 = w.float().abs()
+        ulp = (torch.nextafter(w32, torch.full_like(w32, float("inf"))) - w32).double()
+        err = (lsm[b, :n][fin].double() - w).abs()
+        assert bool((err <= torch.clamp(2 * ulp, min=4e-6)).all()), float((err - torch.clamp(2 * ulp, min=4e-6)).max())
+    lsm_cpu = lsm.cpu()
+    for b, n in enumerate(seq_lens.tolist()):
+        lsm_cpu[b, n:] = 0.0
+    want = cport.decode_alternatives(lsm_cpu.numpy(), seq_lens.numpy(), beam=beam, log_input=True, **cfg)
+    got = dict(tokens=out.numpy(), timesteps=ts.numpy(), scores=scores.numpy(), lens=lens.numpy(),
+               n_results=dec.last_n_results.numpy(), ties=dec.last_flags.numpy())
+    checked, unresolved = compare(want, got, want["ties"], "logits %s %s" % (dtype, cfg))
+    assert checked + unresolved == 3
+    assert not (got["ties"] & FLAG_ERR_ARENA).any()
