@@ -1934,4 +1934,142 @@ CTC_FN void finalize_cta_run(const BeamParams &p, const int b, unsigned char *sm
   }
 }
 
+// ======================================================================================================
+//  committed_cta_run: the committed prefix of one stream -- the path from the root to the lowest common ancestor
+//  (LCA) of the current beam members.  A node's (char, timestep) changes only while its parent is a beam member
+//  (reference path_trie.cpp:38-46) and every future member descends from a current one, so no node on that path
+//  changes, dies or is revived again: its tokens and timesteps start every row any later read-out of the stream
+//  returns.  Trie paths are unique, so the LCA's depth is the longest common prefix of the rows a finalize of the same
+//  state writes.  Reads the state block and the arena only.
+//
+//  The search runs top-down over the jump pointers (Node::jump): every member descends to its ancestor at the
+//  deepest multiple of kJump not below the shallowest member, then all step one jump at a time until their ancestors
+//  agree (at depth 0 all are the root); the last 15 levels above that are resolved by stepping parents in lockstep.
+//  About (depth - LCA depth) / kJump + 2 * kJump dependent hops per member, all members in parallel.  The path
+//  [since, LCA depth) is then written like finalize writes a row: jump checkpoints, stretches in parallel.
+// ======================================================================================================
+constexpr int kCommitCp = 256;  // checkpoints of the write-out per round
+CTC_HD size_t committed_smem_bytes(int K) { return (size_t)K * 3 * 4 + (size_t)kCommitCp * 4 + 64; }
+// since: positions already read out (the previous call's result); outside [0, LCA depth] it is taken as 0.
+// Writes *committed = LCA depth and columns [0, min(depth - since, cap)) of out_tok / out_ts (positions since..).
+template <int NT>
+CTC_FN void committed_cta_run(const Node *nodes, const int *st, int K, int since, int *committed, int *out_tok,
+                              int *out_ts, int cap, unsigned char *smem) {
+  const int M = st[0];
+  const int *s = st + kStateHeader;
+  int *s_cur = (int *)smem;       // [K] each member's ancestor at the current aligned depth
+  int *s_hi = s_cur + K;          // [K] its ancestor one step above that (a checkpoint, or the member's own node)
+  int *s_hd = s_hi + K;           // [K] depth of s_hi
+  int *s_cp = s_hd + K;           // [kCommitCp] write-out checkpoints
+  int *s_ctl = s_cp + kCommitCp;  // [0] -(shallowest member depth), [1] disagreement, [2..4] write-out cursor
+  CTC_PAR {
+    if (tid == 0) { s_ctl[0] = -0x7fffffff; s_ctl[1] = 0; }
+  }
+  CTC_BARRIER();
+  CTC_PAR {
+    for (int j = tid; j < M; j += NT) atom_max_i(&s_ctl[0], -s[2 * K + j]);
+  }
+  CTC_BARRIER();
+  const int dmin = M > 0 ? -s_ctl[0] : 0;
+  int A = dmin / kJump * kJump;
+  CTC_PAR {
+    for (int j = tid; j < M; j += NT) {
+      int nid = s[j], d = s[2 * K + j], hi = nid, hd = d;
+      while (d > A) {
+        hi = nid; hd = d;
+        nid = ld_cg(&nodes[nid].jump);
+        d = (d - 1) / kJump * kJump;
+      }
+      s_cur[j] = nid; s_hi[j] = hi; s_hd[j] = hd;
+    }
+  }
+  CTC_BARRIER();
+  // (a) the deepest aligned depth A at which every member has the same ancestor
+  for (;;) {
+    CTC_PAR {
+      for (int j = tid; j < M; j += NT)
+        if (s_cur[j] != s_cur[0]) s_ctl[1] = 1;  // benign race: all writers store 1
+    }
+    CTC_BARRIER();
+    const int split = s_ctl[1];
+    CTC_BARRIER();  // (everyone has read the flag before it is cleared)
+    if (!split || A == 0) break;
+    CTC_PAR {
+      for (int j = tid; j < M; j += NT) {
+        s_hi[j] = s_cur[j]; s_hd[j] = A;
+        s_cur[j] = ld_cg(&nodes[s_cur[j]].jump);
+      }
+      if (tid == 0) s_ctl[1] = 0;
+    }
+    A -= kJump;
+    CTC_BARRIER();
+  }
+  // (b) the LCA lies in [A, U]: every member's ancestor at depth U, then parents in lockstep until they agree
+  const int U = dmin < A + kJump - 1 ? dmin : A + kJump - 1;
+  CTC_PAR {
+    for (int j = tid; j < M; j += NT) {
+      int nid = s_hi[j];
+      for (int d = s_hd[j]; d > U; --d) nid = ld_cg(&nodes[nid].parent);
+      s_hi[j] = nid;
+    }
+    if (tid == 0) s_ctl[1] = 0;
+  }
+  CTC_BARRIER();
+  int D = U;
+  while (D > A) {
+    CTC_PAR {
+      for (int j = tid; j < M; j += NT)
+        if (s_hi[j] != s_hi[0]) s_ctl[1] = 1;
+    }
+    CTC_BARRIER();
+    const int split = s_ctl[1];
+    CTC_BARRIER();
+    if (!split) break;
+    CTC_PAR {
+      for (int j = tid; j < M; j += NT) s_hi[j] = ld_cg(&nodes[s_hi[j]].parent);
+      if (tid == 0) s_ctl[1] = 0;
+    }
+    --D;
+    CTC_BARRIER();
+  }
+  // (c) write positions [s0, min(D, s0 + cap)) of the path root -> LCA; node of depth d holds position d - 1
+  const int s0 = (since >= 0 && since <= D) ? since : 0;
+  CTC_PAR {
+    if (tid == 0) { *committed = D; s_ctl[2] = M > 0 ? s_hi[0] : 0; s_ctl[3] = D; }
+  }
+  CTC_BARRIER();
+  int dcur = D;
+  while (dcur > s0) {
+    CTC_PAR {
+      if (tid == 0) {
+        int nid = s_ctl[2], d = s_ctl[3], n = 0;
+        while (n < kCommitCp && d > s0) {
+          s_cp[n++] = nid;
+          nid = ld_cg(&nodes[nid].jump);
+          d = (d - 1) / kJump * kJump;
+        }
+        s_ctl[2] = nid; s_ctl[3] = d; s_ctl[4] = n;
+      }
+    }
+    CTC_BARRIER();
+    const int dnext = s_ctl[3], n = s_ctl[4];
+    CTC_PAR {
+      for (int k = tid; k < n; k += NT) {
+        int d = k == 0 ? dcur : (dcur - 1) / kJump * kJump - (k - 1) * kJump;  // depth of the k-th checkpoint
+        int dend = (d - 1) / kJump * kJump;
+        dend = dend > s0 ? dend : s0;
+        int nid = s_cp[k];
+        for (; d > dend; --d) {
+          const Node nd = load_node(&nodes[nid]);
+          const int col = d - 1 - s0;
+          if (col < cap) { out_tok[col] = nd.chr; out_ts[col] = nd.ts; }
+          nid = nd.parent;
+        }
+      }
+    }
+    CTC_BARRIER();
+    dcur = dnext;
+  }
+}
+
 }  // namespace ctc

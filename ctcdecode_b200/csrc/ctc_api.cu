@@ -43,6 +43,62 @@ __global__ void __launch_bounds__(NT) finalize_kernel(const BeamParams p) {
   finalize_cta_run<NT>(p, (int)blockIdx.x, smem);
 }
 
+// committed prefix of a streaming state: one CTA per stream, the stream's arena / state pointers travel in the
+// launch parameters (up to kCommitPerLaunch streams per launch), so the call needs no workspace
+constexpr int kCommitPerLaunch = 192;
+struct CommitArgs {
+  const Node *arena[kCommitPerLaunch];
+  const int *state[kCommitPerLaunch];
+  int K, b0, cap;
+  const int *since;
+  int *committed, *tokens, *timesteps;
+};
+template <int NT>
+__global__ void __launch_bounds__(NT) committed_kernel(const CommitArgs a) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  const int i = (int)blockIdx.x, b = a.b0 + i;
+  committed_cta_run<NT>(a.arena[i], a.state[i], a.K, a.since ? a.since[b] : 0, &a.committed[b],
+                        a.tokens + (size_t)b * a.cap, a.timesteps + (size_t)b * a.cap, a.cap, smem);
+}
+
+// The per-call tables of a streaming chunk (each stream's arena, state block, capacity, eos flag, scorer arrays and
+// chunk length), in device memory.  A kernel writes them from its launch parameters, kTabPerLaunch streams per
+// launch: the call needs no host staging buffer that would have to outlive an asynchronous copy.
+struct StreamTabLayout { size_t arenas, states, caps, fin, lmar, dst, rows, lens, total; };
+static StreamTabLayout stream_tab_layout(int B) {
+  const size_t p = al256((size_t)B * 8), i = al256((size_t)B * 4);
+  StreamTabLayout t;
+  t.arenas = 0; t.states = p; t.caps = 2 * p; t.fin = t.caps + i; t.lmar = t.fin + al256((size_t)B);
+  t.dst = t.lmar + p; t.rows = t.dst + p; t.lens = t.rows + p; t.total = t.lens + i;
+  return t;
+}
+constexpr int kTabPerLaunch = 64;
+struct StreamTabArgs {
+  unsigned char *tab;
+  StreamTabLayout L;
+  int b0, n;
+  Node *arena[kTabPerLaunch];
+  int *state[kTabPerLaunch];
+  float *lmar[kTabPerLaunch];
+  int *dst[kTabPerLaunch];
+  float *rows[kTabPerLaunch];
+  int cap[kTabPerLaunch], len[kTabPerLaunch];
+  unsigned char fin[kTabPerLaunch];
+};
+__global__ void stream_table_kernel(const StreamTabArgs a) {
+  const int i = (int)threadIdx.x;
+  if (i >= a.n) return;
+  const int b = a.b0 + i;
+  reinterpret_cast<Node **>(a.tab + a.L.arenas)[b] = a.arena[i];
+  reinterpret_cast<int **>(a.tab + a.L.states)[b] = a.state[i];
+  reinterpret_cast<int *>(a.tab + a.L.caps)[b] = a.cap[i];
+  a.tab[a.L.fin + b] = a.fin[i];
+  reinterpret_cast<float **>(a.tab + a.L.lmar)[b] = a.lmar[i];
+  reinterpret_cast<int **>(a.tab + a.L.dst)[b] = a.dst[i];
+  reinterpret_cast<float **>(a.tab + a.L.rows)[b] = a.rows[i];
+  reinterpret_cast<int *>(a.tab + a.L.lens)[b] = a.len[i];
+}
+
 __global__ void selftest_math_f64_kernel(int which, const double *x, const double *x2, double *y, size_t n) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
     y[i] = which == 0 ? exp_glibc_nonpos(x[i]) : which == 1 ? log_glibc(x[i]) : lse_d(x[i], x2[i]);
@@ -353,8 +409,16 @@ static void spread_rows(const int *stage_tok, const int *stage_ts, int32_t *toke
   for (auto &th : pool) th.join();
 }
 
+// completion of device-path work (ctcdec_decode_stream_device / ctcdec_stream_committed_device) on a state; one event
+// per call, shared by the call's states
+struct StreamEvent {
+  cudaEvent_t ev = nullptr;
+  ~StreamEvent() { if (ev) cudaEventDestroy(ev); }
+};
+
 // streaming state object
 struct StreamState {
+  std::shared_ptr<StreamEvent> last;  // the last device-path call that used this state (or null)
   ctcdec_config cfg;
   int device;
   Node *arena;
@@ -825,6 +889,7 @@ int ctcdec_state_destroy(void *state) {
   if (!state) return CTCDEC_OK;
   StreamState *st = static_cast<StreamState *>(state);
   cudaSetDevice(st->device);
+  if (st->last) cudaEventSynchronize(st->last->ev);  // device-path work may still read or write the state
   cudaFree(st->arena);
   cudaFree(st->state);
   if (st->lm_arena) cudaFree(st->lm_arena);
@@ -840,143 +905,158 @@ int ctcdec_state_frames(const void *state, int *frames) {
   return CTCDEC_OK;
 }
 
-int ctcdec_decode_stream_host(const float *probs, const int32_t *seq_lens, int B, int T, void *const *states,
-                              const uint8_t *is_eos, int32_t *tokens, int32_t *timesteps, int out_T, float *scores,
-                              int32_t *lens, int32_t *n_results, int32_t *flags) {
-  if (B <= 0) return B == 0 ? CTCDEC_OK : fail(CTCDEC_E_INVALID, "negative batch");
-  if (!states || !is_eos) return fail(CTCDEC_E_INVALID, "states / is_eos is NULL");
+// all states of one call: non-NULL, distinct, same configuration, scorer and device
+static int check_states(void *const *states, int B) {
+  if (!states) return fail(CTCDEC_E_INVALID, "states is NULL");
   for (int b = 0; b < B; ++b)
     if (!states[b]) return fail(CTCDEC_E_INVALID, "states[%d] is NULL", b);
-  StreamState *s0 = static_cast<StreamState *>(states[0]);
-  const ctcdec_config cfg = s0->cfg;
+  const StreamState *s0 = static_cast<const StreamState *>(states[0]);
   for (int b = 1; b < B; ++b) {
-    StreamState *sb = static_cast<StreamState *>(states[b]);
-    if (memcmp(&sb->cfg, &cfg, sizeof(cfg)) != 0 || sb->device != s0->device || sb->sc != s0->sc)
+    const StreamState *sb = static_cast<const StreamState *>(states[b]);
+    if (memcmp(&sb->cfg, &s0->cfg, sizeof(s0->cfg)) != 0 || sb->device != s0->device || sb->sc != s0->sc)
       return fail(CTCDEC_E_UNSUPPORTED, "all states of one call must come from the same decoder configuration, scorer and device");
     for (int a = 0; a < b; ++a)
       if (states[a] == states[b]) return fail(CTCDEC_E_INVALID, "states[%d] and states[%d] are the same object", a, b);
   }
-  Plan pl;
-  int rc = make_plan(&cfg, B, T, &pl);
-  if (rc) return rc;
-  const int device = s0->device;
-  if (cudaSetDevice(device) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "cudaSetDevice(%d) failed", device);
-  if ((rc = check_device())) return rc;
-  std::lock_guard<std::mutex> lock(g_mu[device]);
-  DevCache &c = g_cache[device];
-  if (!c.stream) CU(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
-  cudaStream_t s = c.stream;
-  const int V = cfg.vocab_size, K = cfg.beam_size;
-  bool any_eos = false;
-  int h_len_max = 0;
+  return CTCDEC_OK;
+}
+
+// order work on stream s after the pending device-path calls of these states
+static int wait_device_work(void *const *states, int B, cudaStream_t s) {
+  const StreamEvent *prev = nullptr;
   for (int b = 0; b < B; ++b) {
-    any_eos |= is_eos[b] != 0;
-    int len = seq_lens ? seq_lens[b] : T;
-    len = std::max(0, std::min(len, T));
+    const StreamEvent *e = static_cast<StreamState *>(states[b])->last.get();
+    if (e && e != prev) CU(cudaStreamWaitEvent(s, e->ev, 0));
+    prev = e;
+  }
+  return CTCDEC_OK;
+}
+
+static int record_device_work(void *const *states, int B, cudaStream_t s) {
+  auto e = std::make_shared<StreamEvent>();
+  CU(cudaEventCreateWithFlags(&e->ev, cudaEventDisableTiming));
+  CU(cudaEventRecord(e->ev, s));
+  for (int b = 0; b < B; ++b) static_cast<StreamState *>(states[b])->last = e;
+  return CTCDEC_OK;
+}
+
+// Grow each arena so that 1 + K * (frames consumed after this chunk) nodes fit.  Doubling keeps this to about
+// log2(frames / 256) times per stream; the copy runs on s (after the stream's earlier work) and the host waits for
+// it before the old arrays are freed.
+static int grow_arenas(void *const *states, int B, const int *clen, cudaStream_t s) {
+  for (int b = 0; b < B; ++b) {
     StreamState *sb = static_cast<StreamState *>(states[b]);
-    // grow the arena so that 1 + K * (frames consumed after this chunk) nodes fit
-    const long long need = 1 + (long long)K * (sb->frames + len);
-    if (need > sb->arena_cap) {
-      long long cap = std::max<long long>(need, 2ll * sb->arena_cap);
-      if (cap > 0x7fffffffll / 2) return fail(CTCDEC_E_UNSUPPORTED, "stream too long for the node arena");
-      Node *na = nullptr;
-      CU(cudaMalloc(&na, (size_t)cap * sizeof(Node)));
-      const long long used = std::min<long long>(sb->arena_cap, 1 + (long long)K * sb->frames);
-      CU(cudaMemcpyAsync(na, sb->arena, (size_t)used * sizeof(Node), cudaMemcpyDeviceToDevice, s));
+    const int K = sb->cfg.beam_size, V = sb->cfg.vocab_size;
+    const long long need = 1 + (long long)K * (sb->frames + clen[b]);
+    if (need <= sb->arena_cap) continue;
+    long long cap = std::max<long long>(need, 2ll * sb->arena_cap);
+    if (cap > 0x7fffffffll / 2) return fail(CTCDEC_E_UNSUPPORTED, "stream too long for the node arena");
+    Node *na = nullptr;
+    CU(cudaMalloc(&na, (size_t)cap * sizeof(Node)));
+    const long long used = std::min<long long>(sb->arena_cap, 1 + (long long)K * sb->frames);
+    CU(cudaMemcpyAsync(na, sb->arena, (size_t)used * sizeof(Node), cudaMemcpyDeviceToDevice, s));
+    CU(cudaStreamSynchronize(s));
+    CU(cudaFree(sb->arena));
+    sb->arena = na;
+    if (sb->sc) {
+      float *nl = nullptr;
+      int *nd = nullptr;
+      CU(cudaMalloc(&nl, (size_t)cap * 4));
+      CU(cudaMalloc(&nd, (size_t)cap * 4));
+      CU(cudaMemcpyAsync(nl, sb->lm_arena, (size_t)used * 4, cudaMemcpyDeviceToDevice, s));
+      CU(cudaMemcpyAsync(nd, sb->dstate, (size_t)used * 4, cudaMemcpyDeviceToDevice, s));
       CU(cudaStreamSynchronize(s));
-      CU(cudaFree(sb->arena));
-      sb->arena = na;
-      if (sb->sc) {
-        float *nl = nullptr;
-        int *nd = nullptr;
-        CU(cudaMalloc(&nl, (size_t)cap * 4));
-        CU(cudaMalloc(&nd, (size_t)cap * 4));
-        CU(cudaMemcpyAsync(nl, sb->lm_arena, (size_t)used * 4, cudaMemcpyDeviceToDevice, s));
-        CU(cudaMemcpyAsync(nd, sb->dstate, (size_t)used * 4, cudaMemcpyDeviceToDevice, s));
+      CU(cudaFree(sb->lm_arena));
+      CU(cudaFree(sb->dstate));
+      sb->lm_arena = nl;
+      sb->dstate = nd;
+      if (sb->lm_row) {
+        float *nr = nullptr;
+        CU(cudaMalloc(&nr, (size_t)cap * V * 4));
+        CU(cudaMemcpyAsync(nr, sb->lm_row, (size_t)used * V * 4, cudaMemcpyDeviceToDevice, s));
         CU(cudaStreamSynchronize(s));
-        CU(cudaFree(sb->lm_arena));
-        CU(cudaFree(sb->dstate));
-        sb->lm_arena = nl;
-        sb->dstate = nd;
-        if (sb->lm_row) {
-          float *nr = nullptr;
-          CU(cudaMalloc(&nr, (size_t)cap * V * 4));
-          CU(cudaMemcpyAsync(nr, sb->lm_row, (size_t)used * V * 4, cudaMemcpyDeviceToDevice, s));
-          CU(cudaStreamSynchronize(s));
-          CU(cudaFree(sb->lm_row));
-          sb->lm_row = nr;
-        }
+        CU(cudaFree(sb->lm_row));
+        sb->lm_row = nr;
       }
-      sb->arena_cap = (int)cap;
     }
-    h_len_max = std::max(h_len_max, sb->frames + len);
+    sb->arena_cap = (int)cap;
   }
-  if (any_eos && (!tokens || !timesteps || !scores || !lens)) return fail(CTCDEC_E_INVALID, "an output pointer is NULL");
-  if (any_eos && out_T < 0) return fail(CTCDEC_E_INVALID, "out_T < 0");
-  const size_t n_probs = (size_t)B * T * V, n_bk = (size_t)B * K, n_out = any_eos ? n_bk * (size_t)out_T : 0;
-  const size_t ptr_bytes = al256((size_t)B * 8) * 5 + al256((size_t)B * 4) + al256((size_t)B);
-  HostScorer *const sc = s0->sc;
-  if (sc && (rc = ensure_dict_on_device(sc, device))) return rc;
-  if (sc) pl.L = make_layout(cfg.beam_size, cfg.vocab_size, pl.NP, pl.F, pl.sorted, pl.NT, true);  // + dictionary masks
-  if ((rc = ensure(c, 0, n_probs * 4 + 256))) return rc;
-  if ((rc = ensure(c, 1, (size_t)B * 4 + 256))) return rc;
-  if ((rc = ensure(c, 2, n_out * 4 + 256))) return rc;
-  if ((rc = ensure(c, 3, n_out * 4 + 256))) return rc;
-  if ((rc = ensure(c, 4, n_bk * 4 * 2 + (size_t)B * 8 + 1024))) return rc;
-  if ((rc = ensure(c, 5, pl.off_arena + 512))) return rc;  // only the lp / idx part of the plan is used
-  if ((rc = ensure(c, 6, ptr_bytes + 256))) return rc;
-  float *d_probs = (float *)c.buf[0];
-  int *d_lens_in = seq_lens ? (int *)c.buf[1] : nullptr;
-  int *d_tok = (int *)c.buf[2], *d_ts = (int *)c.buf[3];
-  float *d_scores = (float *)c.buf[4];
-  int *d_lens = (int *)((char *)c.buf[4] + al256(n_bk * 4));
-  int *d_nres = (int *)((char *)d_lens + al256(n_bk * 4));
-  int *d_flags = d_nres + B;
-  // pointer tables
-  std::unique_ptr<unsigned char[]> h_tab(new unsigned char[ptr_bytes]);
-  Node **h_arenas = (Node **)h_tab.get();
-  int **h_states = (int **)(h_tab.get() + al256((size_t)B * 8));
-  int *h_caps = (int *)(h_tab.get() + 2 * al256((size_t)B * 8));
-  unsigned char *h_fin = h_tab.get() + 2 * al256((size_t)B * 8) + al256((size_t)B * 4);
-  const size_t off_lmar = 2 * al256((size_t)B * 8) + al256((size_t)B * 4) + al256((size_t)B);
-  float **h_lmar = (float **)(h_tab.get() + off_lmar);
-  int **h_dst = (int **)(h_tab.get() + off_lmar + al256((size_t)B * 8));
-  float **h_rows = (float **)(h_tab.get() + off_lmar + 2 * al256((size_t)B * 8));
+  return CTCDEC_OK;
+}
+
+// Device buffers of one chunk step.
+struct ChunkBuffers {
+  const void *chunk;  // [B, T, V]: probabilities / log-probabilities (kind IN_F32) or logits
+  int kind;
+  float *lp;          // the plan's pruned rows and characters (a workspace laid out by the plan, up to off_arena)
+  uint16_t *idx;
+  unsigned char *tab; // stream_tab_layout(B).total bytes
+  int32_t *tokens, *timesteps;  // [B, K, out_T]
+  float *scores;                // [B, K]
+  int32_t *lens;                // [B, K]
+  int32_t *n_results, *flags;   // [B]
+  int out_T;
+};
+
+// One chunk step of a streaming decode, enqueued on s; shared by ctcdec_decode_stream_host (which stages the chunk
+// and the results around it) and ctcdec_decode_stream_device.  Grows the arenas, writes the per-call tables, runs the
+// prune scan, the beam kernel (for states with a scorer: the persistent launch with the per-frame host handshake,
+// which needs the pinned exchange buffers of `c` and returns synchronised) and, if a stream is at eos, the finalize
+// kernel; advances every state's frame counter.  n_results / flags are cleared first; flags then collect the prune's
+// and the finalize's bits.
+static int stream_chunk_step(const ctcdec_config &cfg, Plan &pl, void *const *states, int B, int T,
+                             const int32_t *seq_lens, const uint8_t *is_eos, const ChunkBuffers &io, DevCache *c,
+                             cudaStream_t s) {
+  const int V = cfg.vocab_size, K = cfg.beam_size;
+  int rc = CTCDEC_OK;
+  bool any_eos = false;
+  std::vector<int> clen(B);
   for (int b = 0; b < B; ++b) {
-    StreamState *sb = static_cast<StreamState *>(states[b]);
-    h_arenas[b] = sb->arena; h_states[b] = sb->state; h_caps[b] = sb->arena_cap; h_fin[b] = is_eos[b] ? 1 : 0;
-    h_lmar[b] = sb->lm_arena; h_dst[b] = sb->dstate; h_rows[b] = sb->lm_row;
+    clen[b] = std::max(0, std::min(seq_lens ? seq_lens[b] : T, T));
+    any_eos |= is_eos[b] != 0;
   }
-  unsigned char *d_tab = (unsigned char *)c.buf[6];
-  CU(cudaMemcpyAsync(d_tab, h_tab.get(), ptr_bytes, cudaMemcpyHostToDevice, s));
-  if (n_probs) CU(cudaMemcpyAsync(d_probs, probs, n_probs * 4, cudaMemcpyHostToDevice, s));
-  if (seq_lens) CU(cudaMemcpyAsync(d_lens_in, seq_lens, (size_t)B * 4, cudaMemcpyHostToDevice, s));
-  CU(cudaMemsetAsync(d_flags, 0, (size_t)B * 4, s));
-  CU(cudaMemsetAsync(d_nres, 0, (size_t)B * 4, s));
-  unsigned char *ws = (unsigned char *)c.buf[5];
-  ws = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(ws) + 255) / 256 * 256);
-  float *lp = reinterpret_cast<float *>(ws + pl.off_lp);
-  uint16_t *idx = pl.sorted ? reinterpret_cast<uint16_t *>(ws + pl.off_idx) : nullptr;
-  if (T > 0 && (rc = launch_prune(&cfg, pl, PruneInput{d_probs, IN_F32, nullptr, sc != nullptr}, d_lens_in, B, T, lp, idx, d_flags, s))) return rc;
+  if ((rc = grow_arenas(states, B, clen.data(), s))) return rc;
+  HostScorer *const sc = static_cast<StreamState *>(states[0])->sc;
+  if (sc && (rc = ensure_dict_on_device(sc, static_cast<StreamState *>(states[0])->device))) return rc;
+  if (sc) pl.L = make_layout(cfg.beam_size, cfg.vocab_size, pl.NP, pl.F, pl.sorted, pl.NT, true);  // + dictionary masks
+  const StreamTabLayout L = stream_tab_layout(B);
+  for (int b0 = 0; b0 < B; b0 += kTabPerLaunch) {
+    StreamTabArgs a;
+    memset(&a, 0, sizeof(a));
+    a.tab = io.tab; a.L = L; a.b0 = b0; a.n = std::min(kTabPerLaunch, B - b0);
+    for (int i = 0; i < a.n; ++i) {
+      StreamState *sb = static_cast<StreamState *>(states[b0 + i]);
+      a.arena[i] = sb->arena; a.state[i] = sb->state; a.cap[i] = sb->arena_cap; a.fin[i] = is_eos[b0 + i] ? 1 : 0;
+      a.lmar[i] = sb->lm_arena; a.dst[i] = sb->dstate; a.rows[i] = sb->lm_row; a.len[i] = clen[b0 + i];
+    }
+    stream_table_kernel<<<1, kTabPerLaunch, 0, s>>>(a);
+    CU(cudaGetLastError());
+  }
+  const int *d_len = seq_lens ? reinterpret_cast<const int *>(io.tab + L.lens) : nullptr;
+  CU(cudaMemsetAsync(io.flags, 0, (size_t)B * 4, s));
+  CU(cudaMemsetAsync(io.n_results, 0, (size_t)B * 4, s));
+  if (T > 0 && (rc = launch_prune(&cfg, pl, PruneInput{io.chunk, io.kind, nullptr, sc != nullptr}, d_len, B, T, io.lp,
+                                  io.idx, io.flags, s)))
+    return rc;
   BeamParams bp;
   memset(&bp, 0, sizeof(bp));
-  bp.lp = lp; bp.idx = idx; bp.seq_lens = d_lens_in; bp.T = T; bp.V = V; bp.NP = pl.NP; bp.K = K;
+  bp.lp = io.lp; bp.idx = io.idx; bp.seq_lens = d_len; bp.T = T; bp.V = V; bp.NP = pl.NP; bp.K = K;
   bp.blank = cfg.blank_id; bp.tile_frames = pl.F;
-  bp.arena_ptrs = (Node *const *)d_tab; bp.state_ptrs = (int *const *)(d_tab + al256((size_t)B * 8));
-  bp.arena_caps = (const int *)(d_tab + 2 * al256((size_t)B * 8));
-  bp.finalize = d_tab + 2 * al256((size_t)B * 8) + al256((size_t)B * 4);
+  bp.arena_ptrs = (Node *const *)(io.tab + L.arenas); bp.state_ptrs = (int *const *)(io.tab + L.states);
+  bp.arena_caps = (const int *)(io.tab + L.caps);
+  bp.finalize = io.tab + L.fin;
   bp.fresh = 0;
-  bp.out_tokens = d_tok; bp.out_timesteps = d_ts; bp.out_scores = d_scores; bp.out_lens = d_lens;
-  bp.n_results = d_nres; bp.out_T = out_T; bp.flags = d_flags;
+  bp.out_tokens = io.tokens; bp.out_timesteps = io.timesteps; bp.out_scores = io.scores; bp.out_lens = io.lens;
+  bp.n_results = io.n_results; bp.out_T = io.out_T; bp.flags = io.flags;
   if (sc && T > 0) {
     // scorer path: one persistent launch per chunk, hand shake after EVERY frame (the frame after the chunk's last
     // one, in the next call, needs the LM terms of the nodes created now)
     int nls = 0, ups = 0;
     exchange_strides(K, exchange_row_len(*sc), &nls, &ups);
-    if ((rc = ensure_pinned(c, 0, (size_t)B * nls * 4))) return rc;
-    if ((rc = ensure_pinned(c, 1, (size_t)B * ups * 4))) return rc;
-    if ((rc = ensure_pinned(c, 2, 256))) return rc;
-    int *h_newlist = (int *)c.pin[0], *h_upd = (int *)c.pin[1], *hs_abort = (int *)c.pin[2];
+    if ((rc = ensure_pinned(*c, 0, (size_t)B * nls * 4))) return rc;
+    if ((rc = ensure_pinned(*c, 1, (size_t)B * ups * 4))) return rc;
+    if ((rc = ensure_pinned(*c, 2, 256))) return rc;
+    int *h_newlist = (int *)c->pin[0], *h_upd = (int *)c->pin[1], *hs_abort = (int *)c->pin[2];
     for (int b = 0; b < B; ++b) { memset(h_newlist + (size_t)b * nls, 0, 16); memset(h_upd + (size_t)b * ups, 0, 8); }
     if (sc->is_character_based) {  // streams that have not seen a frame yet: the root's row of LM terms first
       std::vector<int> scratch;
@@ -984,23 +1064,19 @@ int ctcdec_decode_stream_host(const float *probs, const int32_t *seq_lens, int B
         if (static_cast<StreamState *>(states[b])->frames == 0)
           lm_char_root_entry(*sc, sc->cond_caches[0], h_upd + (size_t)b * ups, scratch);
       bp.lm_char = 1;
-      bp.lm_row_ptrs = (float *const *)(d_tab + off_lmar + 2 * al256((size_t)B * 8));
+      bp.lm_row_ptrs = (float *const *)(io.tab + L.rows);
     }
     *hs_abort = 0;
     bp.dict_next = sc->d_next; bp.dict_mask = sc->d_mask; bp.dict_wc = sc->dict.wc; bp.dict_start = sc->dict.start;
     bp.space_id = sc->space_id; bp.beta = sc->beta;
-    bp.lm_arena_ptrs = (float *const *)(d_tab + off_lmar);
-    bp.dstate_ptrs = (int *const *)(d_tab + off_lmar + al256((size_t)B * 8));
+    bp.lm_arena_ptrs = (float *const *)(io.tab + L.lmar);
+    bp.dstate_ptrs = (int *const *)(io.tab + L.dst);
     bp.newlist = h_newlist; bp.lm_upd = h_upd; bp.lm_nl_stride = nls; bp.lm_up_stride = ups;
     bp.lm_persistent = 1; bp.lm_hs_last = 1; bp.hs_abort = hs_abort;
     if ((rc = launch_beam(bp, pl, B, s))) return rc;
     std::vector<TrieMirror *> mirrors(B);
-    std::vector<int> answers(B);
-    for (int b = 0; b < B; ++b) {
-      mirrors[b] = &static_cast<StreamState *>(states[b])->mirror;
-      answers[b] = std::max(0, std::min(seq_lens ? seq_lens[b] : T, T));
-    }
-    const int failed = serve_handshakes(sc, B, K, answers.data(), mirrors.data(), h_newlist, h_upd, nullptr);
+    for (int b = 0; b < B; ++b) mirrors[b] = &static_cast<StreamState *>(states[b])->mirror;
+    const int failed = serve_handshakes(sc, B, K, clen.data(), mirrors.data(), h_newlist, h_upd, nullptr);
     if (failed) reinterpret_cast<std::atomic<int> *>(hs_abort)->store(1, std::memory_order_release);
     const cudaError_t e = cudaStreamSynchronize(s);
     if (e != cudaSuccess) return fail(CTCDEC_E_CUDA, "beam kernel (scorer path, streaming): %s", cudaGetErrorString(e));
@@ -1008,12 +1084,61 @@ int ctcdec_decode_stream_host(const float *probs, const int32_t *seq_lens, int B
   } else if (T > 0 && (rc = launch_beam(bp, pl, B, s))) {
     return rc;
   }
-  for (int b = 0; b < B; ++b) {
-    int len = seq_lens ? seq_lens[b] : T;
-    static_cast<StreamState *>(states[b])->frames += std::max(0, std::min(len, T));
-  }
+  for (int b = 0; b < B; ++b) static_cast<StreamState *>(states[b])->frames += clen[b];
+  if (any_eos && (rc = launch_finalize(bp, B, s))) return rc;
+  return CTCDEC_OK;
+}
+
+int ctcdec_decode_stream_host(const float *probs, const int32_t *seq_lens, int B, int T, void *const *states,
+                              const uint8_t *is_eos, int32_t *tokens, int32_t *timesteps, int out_T, float *scores,
+                              int32_t *lens, int32_t *n_results, int32_t *flags) {
+  if (B <= 0) return B == 0 ? CTCDEC_OK : fail(CTCDEC_E_INVALID, "negative batch");
+  if (!states || !is_eos) return fail(CTCDEC_E_INVALID, "states / is_eos is NULL");
+  int rc = check_states(states, B);
+  if (rc) return rc;
+  StreamState *s0 = static_cast<StreamState *>(states[0]);
+  const ctcdec_config cfg = s0->cfg;
+  Plan pl;
+  if ((rc = make_plan(&cfg, B, T, &pl))) return rc;
+  const int device = s0->device;
+  if (cudaSetDevice(device) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "cudaSetDevice(%d) failed", device);
+  if ((rc = check_device())) return rc;
+  std::lock_guard<std::mutex> lock(g_mu[device]);
+  DevCache &c = g_cache[device];
+  if (!c.stream) CU(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
+  cudaStream_t s = c.stream;
+  if ((rc = wait_device_work(states, B, s))) return rc;
+  const int V = cfg.vocab_size, K = cfg.beam_size;
+  bool any_eos = false;
+  for (int b = 0; b < B; ++b) any_eos |= is_eos[b] != 0;
+  if (any_eos && (!tokens || !timesteps || !scores || !lens)) return fail(CTCDEC_E_INVALID, "an output pointer is NULL");
+  if (any_eos && out_T < 0) return fail(CTCDEC_E_INVALID, "out_T < 0");
+  const size_t n_probs = (size_t)B * T * V, n_bk = (size_t)B * K, n_out = any_eos ? n_bk * (size_t)out_T : 0;
+  HostScorer *const sc = s0->sc;
+  if ((rc = ensure(c, 0, n_probs * 4 + 256))) return rc;
+  if ((rc = ensure(c, 2, n_out * 4 + 256))) return rc;
+  if ((rc = ensure(c, 3, n_out * 4 + 256))) return rc;
+  if ((rc = ensure(c, 4, n_bk * 4 * 2 + (size_t)B * 8 + 1024))) return rc;
+  if ((rc = ensure(c, 5, pl.off_arena + 512))) return rc;  // only the lp / idx part of the plan is used
+  if ((rc = ensure(c, 6, stream_tab_layout(B).total + 256))) return rc;
+  float *d_probs = (float *)c.buf[0];
+  int *d_tok = (int *)c.buf[2], *d_ts = (int *)c.buf[3];
+  float *d_scores = (float *)c.buf[4];
+  int *d_lens = (int *)((char *)c.buf[4] + al256(n_bk * 4));
+  int *d_nres = (int *)((char *)d_lens + al256(n_bk * 4));
+  int *d_flags = d_nres + B;
+  if (n_probs) CU(cudaMemcpyAsync(d_probs, probs, n_probs * 4, cudaMemcpyHostToDevice, s));
+  unsigned char *ws = (unsigned char *)c.buf[5];
+  ws = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(ws) + 255) / 256 * 256);
+  ChunkBuffers io;
+  io.chunk = d_probs; io.kind = IN_F32;
+  io.lp = reinterpret_cast<float *>(ws + pl.off_lp);
+  io.idx = pl.sorted ? reinterpret_cast<uint16_t *>(ws + pl.off_idx) : nullptr;
+  io.tab = (unsigned char *)c.buf[6];
+  io.tokens = d_tok; io.timesteps = d_ts; io.scores = d_scores; io.lens = d_lens; io.n_results = d_nres;
+  io.flags = d_flags; io.out_T = out_T;
+  if ((rc = stream_chunk_step(cfg, pl, states, B, T, seq_lens, is_eos, io, &c, s))) return rc;
   if (any_eos) {
-    if ((rc = launch_finalize(bp, B, s))) return rc;
     std::unique_ptr<int[]> h_nres(new int[(size_t)B * 2]);
     std::unique_ptr<float[]> h_scores(new float[n_bk]);
     std::unique_ptr<int[]> h_lens(new int[n_bk]);
@@ -1056,6 +1181,105 @@ int ctcdec_decode_stream_host(const float *probs, const int32_t *seq_lens, int B
     if (n_results) memset(n_results, 0, (size_t)B * 4);
   }
   return CTCDEC_OK;
+}
+
+// device scratch of ctcdec_decode_stream_device: the plan's pruned rows / characters, then the per-call tables
+static size_t stream_workspace_bytes(const Plan &pl, int B) { return al256(pl.off_arena) + stream_tab_layout(B).total + 256; }
+
+int ctcdec_stream_workspace_bytes(const ctcdec_config *cfg, int B, int T, size_t *bytes) {
+  Plan pl;
+  int rc = make_plan(cfg, B, T, &pl);
+  if (rc) return rc;
+  if (!bytes) return fail(CTCDEC_E_INVALID, "bytes is NULL");
+  *bytes = stream_workspace_bytes(pl, B);
+  return CTCDEC_OK;
+}
+
+// the states' device must be the current one: the caller's stream and buffers belong to it
+static int check_current_device(const StreamState *s0) {
+  int dev = -1;
+  if (cudaGetDevice(&dev) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "no CUDA device (this library has no CPU fallback)");
+  if (dev != s0->device) return fail(CTCDEC_E_INVALID, "the states live on device %d, the current device is %d", s0->device, dev);
+  return check_device();
+}
+
+int ctcdec_decode_stream_device(const void *probs, int dtype, const int32_t *seq_lens, int B, int T,
+                                void *const *states, const uint8_t *is_eos, int32_t *tokens, int32_t *timesteps,
+                                int out_T, float *scores, int32_t *lens, int32_t *n_results, int32_t *flags,
+                                void *workspace, size_t workspace_bytes, void *stream) {
+  if (B <= 0) return B == 0 ? CTCDEC_OK : fail(CTCDEC_E_INVALID, "negative batch");
+  if (dtype != -1 && dtype != CTCDEC_DTYPE_F32 && dtype != CTCDEC_DTYPE_F16 && dtype != CTCDEC_DTYPE_BF16)
+    return fail(CTCDEC_E_INVALID, "dtype %d is not -1 (probabilities) or one of CTCDEC_DTYPE_F32 / F16 / BF16", dtype);
+  const int kind = dtype == -1 ? IN_F32 : dtype == CTCDEC_DTYPE_F32 ? IN_LOGITS_F32
+                 : dtype == CTCDEC_DTYPE_F16 ? IN_LOGITS_F16 : IN_LOGITS_BF16;
+  if (!states || !is_eos) return fail(CTCDEC_E_INVALID, "states / is_eos is NULL");
+  int rc = check_states(states, B);
+  if (rc) return rc;
+  StreamState *s0 = static_cast<StreamState *>(states[0]);
+  if (s0->sc)
+    return fail(CTCDEC_E_UNSUPPORTED, "states with a scorer need the per-frame host handshake: use ctcdec_decode_stream_host");
+  const ctcdec_config cfg = s0->cfg;
+  Plan pl;
+  if ((rc = make_plan(&cfg, B, T, &pl))) return rc;
+  if (!probs && T > 0) return fail(CTCDEC_E_INVALID, "probs is NULL");
+  if (!n_results || !flags) return fail(CTCDEC_E_INVALID, "n_results and flags device buffers are required");
+  bool any_eos = false;
+  for (int b = 0; b < B; ++b) {
+    if (!is_eos[b]) continue;
+    any_eos = true;
+    const int len = std::max(0, std::min(seq_lens ? seq_lens[b] : T, T));
+    const int need = static_cast<StreamState *>(states[b])->frames + len;
+    if (out_T < need) return fail(CTCDEC_E_INVALID, "out_T (%d) smaller than stream %d's frames after this chunk (%d)", out_T, b, need);
+  }
+  if (any_eos && (!tokens || !timesteps || !scores || !lens)) return fail(CTCDEC_E_INVALID, "an output pointer is NULL");
+  if ((rc = check_current_device(s0))) return rc;
+  unsigned char *ws = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(workspace) + 255) / 256 * 256);
+  const size_t need = stream_workspace_bytes(pl, B);
+  if (!workspace || workspace_bytes < need)
+    return fail(CTCDEC_E_WORKSPACE, "workspace of %zu bytes given, %zu needed", workspace_bytes, need);
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  std::lock_guard<std::mutex> lock(g_mu[s0->device]);
+  if ((rc = wait_device_work(states, B, s))) return rc;
+  ChunkBuffers io;
+  io.chunk = probs; io.kind = kind;
+  io.lp = reinterpret_cast<float *>(ws + pl.off_lp);
+  io.idx = pl.sorted ? reinterpret_cast<uint16_t *>(ws + pl.off_idx) : nullptr;
+  io.tab = ws + al256(pl.off_arena);
+  io.tokens = tokens; io.timesteps = timesteps; io.scores = scores; io.lens = lens; io.n_results = n_results;
+  io.flags = flags; io.out_T = out_T;
+  if ((rc = stream_chunk_step(cfg, pl, states, B, T, seq_lens, is_eos, io, nullptr, s))) return rc;
+  return record_device_work(states, B, s);
+}
+
+int ctcdec_stream_committed_device(void *const *states, int B, const int32_t *since, int32_t *committed,
+                                   int32_t *tokens, int32_t *timesteps, int cap, void *stream) {
+  if (B <= 0) return B == 0 ? CTCDEC_OK : fail(CTCDEC_E_INVALID, "negative batch");
+  if (!committed) return fail(CTCDEC_E_INVALID, "committed is NULL");
+  if (cap < 0) return fail(CTCDEC_E_INVALID, "cap %d < 0", cap);
+  if (cap > 0 && (!tokens || !timesteps)) return fail(CTCDEC_E_INVALID, "tokens / timesteps is NULL");
+  int rc = check_states(states, B);
+  if (rc) return rc;
+  StreamState *s0 = static_cast<StreamState *>(states[0]);
+  if ((rc = check_current_device(s0))) return rc;
+  const int K = s0->cfg.beam_size;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  std::lock_guard<std::mutex> lock(g_mu[s0->device]);
+  if ((rc = wait_device_work(states, B, s))) return rc;
+  const size_t smem = committed_smem_bytes(K);
+  if (smem > 48 * 1024) CU(cudaFuncSetAttribute(committed_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  for (int b0 = 0; b0 < B; b0 += kCommitPerLaunch) {
+    CommitArgs a;
+    memset(&a, 0, sizeof(a));
+    const int n = std::min(kCommitPerLaunch, B - b0);
+    for (int i = 0; i < n; ++i) {
+      const StreamState *sb = static_cast<const StreamState *>(states[b0 + i]);
+      a.arena[i] = sb->arena; a.state[i] = sb->state;
+    }
+    a.K = K; a.b0 = b0; a.cap = cap; a.since = since; a.committed = committed; a.tokens = tokens; a.timesteps = timesteps;
+    committed_kernel<128><<<n, 128, smem, s>>>(a);
+    CU(cudaGetLastError());
+  }
+  return record_device_work(states, B, s);
 }
 
 // ---------------------------------------------------------------------------------------------------

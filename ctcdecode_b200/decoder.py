@@ -20,6 +20,9 @@ Differences from the reference, all additive:
   * the [batch, beam, T] result tensors are PAGE-LOCKED CPU tensors (torch's caching host allocator, so a decode loop
     reuses the same blocks) up to CTCDECODE_B200_PIN_OUTPUT_BYTES per tensor (default 1 GiB), pageable beyond: a fresh
     pageable [256, 100, 1000] int32 pair costs page faults on every call, several times the decode itself.
+  * ``OnlineCTCBeamDecoder``: CUDA chunks (without a scorer) are decoded in place on the current stream, raw logits go
+    through ``decode_logits``, ``device_outputs=True`` leaves the results on the GPU, and ``committed_prefix`` reports
+    the part of each stream's transcript no later chunk can change.
   * ``device="all"`` (or no device and a CPU batch of more than 4 x 132 utterances on a multi-GPU box): the host batch
     is sharded over every visible GPU by one call (ctcdec_decode_batch_host_multi).
 """
@@ -269,8 +272,11 @@ class OnlineCTCBeamDecoder(_Base):
     DecoderState (beam, trie, absolute frame counter) lives in GPU memory between chunks."""
 
     def __init__(self, labels, model_path=None, alpha=0, beta=0, cutoff_top_n=40, cutoff_prob=1.0, beam_width=100,
-                 num_processes=4, blank_id=0, log_probs_input=False, device=None, scorer_provider=None):
+                 num_processes=4, blank_id=0, log_probs_input=False, device=None, scorer_provider=None,
+                 device_outputs=False):
         self._cutoff_top_n = cutoff_top_n  # private name kept from the reference (:175)
+        self._device_outputs = device_outputs
+        self._ws = None
         self._init_common(labels, model_path, alpha, beta, cutoff_top_n, cutoff_prob, beam_width, num_processes,
                           blank_id, log_probs_input, device, scorer_provider=scorer_provider)
 
@@ -280,14 +286,20 @@ class OnlineCTCBeamDecoder(_Base):
     def decode(self, probs, states, is_eos_s, seq_lens=None):
         """Feeds one chunk per stream.  Returns (beam_results, beam_scores, timesteps, out_lens) like reference
         __init__.py:189-238: beam_results / timesteps are [B, n_beams, max_len] (both [B, 0, 0] while no stream
-        has reached eos), beam_scores / out_lens are [B, beam]."""
+        has reached eos), beam_scores / out_lens are [B, beam].
+
+        A CUDA chunk (without a scorer) is decoded in place on the current stream (ctcdec_decode_stream_device).
+        With device_outputs=True the results stay on the GPU and the call does not wait for it: beam_results /
+        timesteps are [B, beam, out_T] (out_T: the most frames an eos stream has consumed; [B, 0, 0] without eos),
+        only [b, p, :out_lens[b, p]] of rows p < last_n_results[b] of eos streams being meaningful."""
         lib = _native.load()
+        if probs.dim() != 3:
+            raise ValueError("probs must be [batch, time, labels], got %s" % (tuple(probs.shape),))
+        if probs.is_cuda and self._scorer is None:
+            return self._decode_device(lib, probs, states, is_eos_s, seq_lens, -1)
         probs = probs.cpu().float().contiguous()
         B, T, V = probs.shape
-        if V != self._num_labels:
-            raise ValueError("probs has %d labels, decoder was built with %d" % (V, self._num_labels))
-        if len(states) != B or len(is_eos_s) != B:
-            raise ValueError("need one state and one is_eos flag per batch item")
+        self._check_chunk(B, V, states, is_eos_s)
         if seq_lens is not None:
             seq_lens = seq_lens.cpu().int().contiguous()
         K = self._beam_width
@@ -322,6 +334,134 @@ class OnlineCTCBeamDecoder(_Base):
         return (tokens[:, :max_res, :max_len].contiguous(), scores, timesteps[:, :max_res, :max_len].contiguous(),
                 out_seq_len)
 
+    def decode_logits(self, logits, states, is_eos_s, seq_lens=None):
+        """Extension: decode's CUDA path for the acoustic model's raw LOGITS, a CUDA tensor [B, T, V] in float32 /
+        float16 / bfloat16; each frame's float32 log-softmax is taken on the fly (as CTCBeamDecoder.decode_logits
+        does), so chunks decode exactly like the concatenated logits would offline."""
+        lib = _native.load()
+        if self._scorer is not None:
+            raise NotImplementedError("ctcdecode_b200: decode_logits with a scorer is not built")
+        if logits.dim() != 3 or not logits.is_cuda:
+            raise ValueError("logits must be a CUDA tensor [batch, time, labels]")
+        dtypes = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
+        if logits.dtype not in dtypes:
+            raise ValueError("logits must be float32, float16 or bfloat16, got %s" % logits.dtype)
+        return self._decode_device(lib, logits, states, is_eos_s, seq_lens, dtypes[logits.dtype])
+
+    def _check_chunk(self, B, V, states, is_eos_s):
+        if V != self._num_labels:
+            raise ValueError("probs has %d labels, decoder was built with %d" % (V, self._num_labels))
+        if len(states) != B or len(is_eos_s) != B:
+            raise ValueError("need one state and one is_eos flag per batch item")
+
+    @staticmethod
+    def _frames(lib, states):
+        out = []
+        for s in states:
+            fr = ctypes.c_int(0)
+            _native.check(lib.ctcdec_state_frames(s.state, ctypes.byref(fr)))
+            out.append(fr.value)
+        return out
+
+    @staticmethod
+    def _states_device(states, dev):
+        for s in states:
+            if s.device != dev.index:
+                raise ValueError("a state lives on cuda:%d, the chunk on %s" % (s.device, dev))
+
+    def _decode_device(self, lib, x, states, is_eos_s, seq_lens, dtype):
+        B, T, V = x.shape
+        self._check_chunk(B, V, states, is_eos_s)
+        dev = x.device
+        self._states_device(states, dev)
+        x = (x.float() if dtype < 0 else x).contiguous()
+        # seq_lens, is_eos and the frame counts stay on the host: the output sizes follow without reading the device
+        lens_h = [T] * B if seq_lens is None else [max(0, min(int(v), T)) for v in seq_lens.cpu().tolist()]
+        sl = None if seq_lens is None else torch.tensor(lens_h, dtype=torch.int32)
+        eos = [bool(e) for e in is_eos_s]
+        eos_b = [b for b in range(B) if eos[b]]
+        frames = self._frames(lib, [states[b] for b in eos_b])
+        out_T = max([frames[i] + lens_h[b] for i, b in enumerate(eos_b)], default=0)
+        K = self._beam_width
+        cfg = _cfg(self)
+        nbytes = ctypes.c_size_t(0)
+        _native.check(lib.ctcdec_stream_workspace_bytes(ctypes.byref(cfg), B, T, ctypes.byref(nbytes)))
+        if self._ws is None or self._ws.numel() < nbytes.value or self._ws.device != dev:
+            self._ws = None
+            self._ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        tokens = torch.zeros(B, K, max(out_T, 1), dtype=torch.int32, device=dev)
+        timesteps = torch.zeros(B, K, max(out_T, 1), dtype=torch.int32, device=dev)
+        scores = torch.zeros(B, K, dtype=torch.float32, device=dev)
+        out_seq_len = torch.zeros(B, K, dtype=torch.int32, device=dev)
+        n_results = torch.zeros(B, dtype=torch.int32, device=dev)
+        flags = torch.zeros(B, dtype=torch.int32, device=dev)
+        handles = (ctypes.c_void_p * B)(*[s.state for s in states])
+        eos_arr = (ctypes.c_uint8 * B)(*[1 if e else 0 for e in eos])
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            _native.check(lib.ctcdec_decode_stream_device(
+                x.data_ptr(), dtype, sl.data_ptr() if sl is not None else None, B, T, handles, eos_arr,
+                tokens.data_ptr(), timesteps.data_ptr(), max(out_T, 1), scores.data_ptr(), out_seq_len.data_ptr(),
+                n_results.data_ptr(), flags.data_ptr(), self._ws.data_ptr(), self._ws.numel(), stream))
+        if self._device_outputs:
+            self.last_flags, self.last_n_results = flags, n_results
+            if not any(eos):
+                empty = torch.zeros(B, 0, 0, dtype=torch.int32, device=dev)
+                return empty, scores, empty.clone(), out_seq_len
+            return tokens[:, :, :out_T], scores, timesteps[:, :, :out_T], out_seq_len
+        # the host path's return values: CPU tensors, [B, max_res, max_len] (flags are not reported without eos)
+        n_results, lens_cpu = n_results.cpu(), out_seq_len.cpu()
+        flags = flags.cpu() if any(eos) else torch.zeros(B, dtype=torch.int32)
+        self.last_flags, self.last_n_results = flags, n_results
+        if (flags & _native.FLAG_ERR_ARENA).any():
+            raise _native.NativeError("ctcdecode_b200: the beam kernel reported an internal error (node arena "
+                                      "exhausted); results are not valid")
+        if not any(eos):
+            empty = torch.zeros(B, 0, 0, dtype=torch.int32)
+            return empty, scores.cpu(), empty.clone(), lens_cpu
+        max_res, max_len = int(n_results.max()), int(lens_cpu.max())
+        return (tokens[:, :max_res, :max_len].cpu(), scores.cpu(), timesteps[:, :max_res, :max_len].cpu(), lens_cpu)
+
+    def committed_prefix(self, states, since=None):
+        """Extension: the part of each stream's transcript that no later chunk can change -- the path from the trie
+        root to the lowest common ancestor of the stream's beam members (ctcdec_stream_committed_device).  Its tokens
+        and timesteps start every row any later decode of the stream returns.  since: int32 [B] positions the caller
+        already has (normally the previous call's `committed`), None = 0; a value beyond the committed depth reads
+        from 0.  Returns (tokens [B, D], timesteps [B, D], n_new [B], committed [B]): row b holds the n_new[b] new
+        positions from column 0, D = max(n_new).  CUDA tensors with device_outputs=True, CPU tensors otherwise; the
+        call waits for the device once, to size D."""
+        lib = _native.load()
+        B = len(states)
+        if B == 0:
+            z = torch.zeros(0, dtype=torch.int32)
+            return z.view(0, 0), z.view(0, 0), z, z
+        devs = {s.device for s in states}
+        if len(devs) != 1:
+            raise ValueError("all states must live on one device, got %s" % sorted(devs))
+        dev = torch.device("cuda", devs.pop())
+        cap = max(max(self._frames(lib, states)), 1)  # committed <= frames consumed: nothing is cut off
+        tok = torch.empty(B, cap, dtype=torch.int32, device=dev)
+        ts = torch.empty(B, cap, dtype=torch.int32, device=dev)
+        committed = torch.empty(B, dtype=torch.int32, device=dev)
+        if since is not None:
+            since = torch.as_tensor(since).to(device=dev, dtype=torch.int32).contiguous()
+            if since.shape != (B,):
+                raise ValueError("since must be [batch]")
+        handles = (ctypes.c_void_p * B)(*[s.state for s in states])
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            _native.check(lib.ctcdec_stream_committed_device(
+                handles, B, since.data_ptr() if since is not None else None, committed.data_ptr(), tok.data_ptr(),
+                ts.data_ptr(), cap, stream))
+        start = torch.zeros_like(committed) if since is None else \
+            torch.where((since >= 0) & (since <= committed), since, torch.zeros_like(since))
+        n_new = committed - start
+        D = int(n_new.max())
+        tok, ts = tok[:, :D], ts[:, :D]
+        if self._device_outputs:
+            return tok, ts, n_new, committed
+        return tok.cpu(), ts.cpu(), n_new.cpu(), committed.cpu()
+
     def reset_state(state):  # noqa: N805 -- signature kept from the reference (:249), which lacks `self`
         state.release()
 
@@ -336,8 +476,8 @@ class DecoderState(object):
         # the scorer is borrowed by the state (reference ctc_beam_search_decoder.cpp:31): keep the decoder alive
         self._decoder = decoder
         scorer = decoder._scorer.handle if decoder._scorer else None
-        _native.check(lib.ctcdec_state_create_lm(ctypes.byref(cfg), scorer, decoder._device_index(),
-                                                 ctypes.byref(handle)))
+        self.device = decoder._device_index()
+        _native.check(lib.ctcdec_state_create_lm(ctypes.byref(cfg), scorer, self.device, ctypes.byref(handle)))
         self.state = handle.value
 
     def release(self):

@@ -200,6 +200,49 @@ int ctcdec_decode_stream_host(const float *probs, const int32_t *seq_lens, int B
                               const uint8_t *is_eos, int32_t *tokens, int32_t *timesteps, int out_T, float *scores,
                               int32_t *lens, int32_t *n_results, int32_t *flags);
 
+/* Bytes of device scratch one ctcdec_decode_stream_device call of B streams and T frames needs (the pruned rows of
+ * the chunk and the per-call tables of stream pointers). */
+int ctcdec_stream_workspace_bytes(const ctcdec_config *cfg, int B, int T, size_t *bytes);
+
+/* ctcdec_decode_stream_host with the chunk and the results on the DEVICE, enqueued on `stream` (a cudaStream_t of the
+ * states' device, which must be the current device).  Extension: the reference decodes CPU tensors only.
+ *   probs      [B, T, V] device buffer.  dtype -1: float32 probabilities, or log-probabilities if cfg->log_input;
+ *              CTCDEC_DTYPE_F32 / F16 / BF16: raw logits, log-softmaxed per frame by the scan kernel as in
+ *              ctcdec_decode_batch_device_logits (cfg->log_input is ignored).
+ *   seq_lens   HOST int32 [B] or NULL; is_eos and states are host arrays too.  The host therefore knows every
+ *              stream's frame count: ctcdec_state_frames is exact as soon as the call returns.
+ *   tokens / timesteps [B, beam, out_T], scores / lens [B, beam]: device buffers, written for eos streams only (rows
+ *              p < n_results[b]); out_T must be >= frames consumed after this chunk by every eos stream (checked).
+ *   n_results / flags [B]: device buffers, required.  Every entry is written: n_results 0 for streams not at eos,
+ *              flags the CTCDEC_FLAG_* bits of this chunk (and of the finalize for eos streams).  A set
+ *              CTCDEC_FLAG_ERR_ARENA means the stream's results are not valid; this call cannot report it as an error
+ *              code without waiting for the kernels.
+ * The call does not wait for the device, with one exception: when a stream's node arena must grow (1 + beam x frames
+ * nodes, capacity doubling from 256 frames: about log2(frames / 256) times per stream) the old arena is copied on
+ * `stream` and the host waits for that copy before freeing it.  States with a scorer return CTCDEC_E_UNSUPPORTED
+ * (their beam kernel needs the per-frame host handshake of ctcdec_decode_stream_host).  The workspace and the outputs
+ * must not be reused before the work on `stream` is done, as with ctcdec_decode_batch_device.
+ * Device-path calls record an event on each state; ctcdec_decode_stream_host waits for it on its own stream, a later
+ * device-path call on another stream waits for it too, and ctcdec_state_destroy synchronises it before freeing. */
+int ctcdec_decode_stream_device(const void *probs, int dtype, const int32_t *seq_lens, int B, int T,
+                                void *const *states, const uint8_t *is_eos, int32_t *tokens, int32_t *timesteps,
+                                int out_T, float *scores, int32_t *lens, int32_t *n_results, int32_t *flags,
+                                void *workspace, size_t workspace_bytes, void *stream);
+
+/* Extension: the COMMITTED prefix of every stream -- the part of the transcript no later chunk can change.  It is the
+ * trie path from the root to the lowest common ancestor of the stream's current beam members: the longest common
+ * prefix of the rows an eos read-out would return now, which also starts every row of any later read-out, tokens and
+ * timesteps alike (DESIGN.md, "Streaming on the device").
+ *   committed  device int32 [B]: the committed depth (never decreases from chunk to chunk);
+ *   since      device int32 [B] or NULL (= 0): positions the caller already has, normally the previous call's
+ *              committed[b].  A value outside [0, committed depth] is taken as 0;
+ *   tokens / timesteps  device int32 [B, cap]: row b receives positions [since[b], committed[b]) from column 0;
+ *              columns at or beyond cap are not written (compare committed - since with cap).
+ * Reads the states only, so any state works, including one with a scorer advanced by ctcdec_decode_stream_host.
+ * Enqueued on `stream` (the states' device must be the current device); does not wait for the device. */
+int ctcdec_stream_committed_device(void *const *states, int B, const int32_t *since, int32_t *committed,
+                                   int32_t *tokens, int32_t *timesteps, int cap, void *stream);
+
 /* ---- measurement hook (bench.py) --------------------------------------------------------------------
  * With profiling enabled on the calling thread, ctcdec_decode_batch_device records CUDA events on its stream
  * around each of its three kernels; ctcdec_profile_read waits for the last decode of this thread and returns
