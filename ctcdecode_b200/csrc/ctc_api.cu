@@ -151,11 +151,12 @@ static int check_error_flags(const int *flags, int B) {
   return CTCDEC_OK;
 }
 
-static int make_plan(const ctcdec_config *cfg, int B, int T, Plan *pl) {
+// lm: a scorer is attached (pl->L is then the scorer kernel's layout)
+static int make_plan(const ctcdec_config *cfg, int B, int T, Plan *pl, bool lm = false) {
   char msg[256];
   int nt = 0;
   if (const char *e = getenv("CTCDEC_NT")) nt = atoi(e);  // tuning knob: threads per CTA of the beam kernel
-  const int rc = make_plan_core(cfg, B, T, pl, msg, sizeof(msg), nt, g_batch_in_flight);
+  const int rc = make_plan_core(cfg, B, T, pl, msg, sizeof(msg), nt, g_batch_in_flight, lm);
   if (rc) return fail(rc, "%s", msg);
   return CTCDEC_OK;
 }
@@ -281,21 +282,17 @@ static int launch_prune(const ctcdec_config *cfg, const Plan &pl, const PruneInp
   pp.want_blank_prob = in.blank_prob ? 1 : 0;
   const int V = cfg->vocab_size;
   pp.Vpad = (V + 3) / 4 * 4;
-  const size_t row_bytes = logits ? (size_t)pp.Vpad * 4 : 0;  // per-warp staging row of the log-softmax
   const long long frames = (long long)B * T;
   if (frames == 0) return CTCDEC_OK;
   int rc = CTCDEC_OK;
+  const PruneShape ps = prune_shape(pl, V, logits);
+  const int wpc = ps.wpc;
+  const size_t smem = ps.smem;
   if (!pl.sorted) {
-    int wpc = 8;
-    if (logits) wpc = (int)std::max<size_t>(1, std::min<size_t>(8, (200 * 1024 - 2048) / row_bytes));
-    const size_t smem = 2048 + (size_t)wpc * row_bytes;
     const int grid = (int)std::min<long long>((frames + wpc - 1) / wpc, kNumSMs * 16);
     rc = logits ? launch_prune_k<false, 0, true>(pp, grid, wpc * 32, smem, s)
                 : launch_prune_k<false, 0, false>(pp, grid, wpc * 32, smem, s);
   } else {
-    int wpc = (int)std::min<size_t>(8, (200 * 1024 - 2048) / ((size_t)pl.P * 8 + row_bytes));
-    if (wpc < 1) wpc = 1;
-    const size_t smem = 2048 + (size_t)wpc * ((size_t)pl.P * 8 + row_bytes);
     const int grid = (int)std::min<long long>((frames + wpc - 1) / wpc, kNumSMs * 8);
     if (V <= 256)
       rc = logits ? launch_prune_k<true, 8, true>(pp, grid, wpc * 32, smem, s) : launch_prune_k<true, 8, false>(pp, grid, wpc * 32, smem, s);
@@ -837,9 +834,11 @@ static int state_init_device(StreamState *st) {
   return CTCDEC_OK;
 }
 
-int ctcdec_state_create(const ctcdec_config *cfg, int device, void **state) {
+// lm: the state will decode with a scorer, whose beam kernel layout is checked instead (at one stream, the widest
+// block size the plan picks for the configuration: every batch of such states fits then)
+static int state_create(const ctcdec_config *cfg, int device, bool lm, void **state) {
   Plan pl;
-  int rc = make_plan(cfg, 1, 1, &pl);
+  int rc = make_plan(cfg, 1, 1, &pl, lm);
   if (rc) return rc;
   if (!state) return fail(CTCDEC_E_INVALID, "state is NULL");
   if (cudaSetDevice(device) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "cudaSetDevice(%d) failed (this library has no CPU fallback)", device);
@@ -858,12 +857,14 @@ int ctcdec_state_create(const ctcdec_config *cfg, int device, void **state) {
   return CTCDEC_OK;
 }
 
+int ctcdec_state_create(const ctcdec_config *cfg, int device, void **state) { return state_create(cfg, device, false, state); }
+
 int ctcdec_state_create_lm(const ctcdec_config *cfg, void *scorer, int device, void **state) {
   if (!scorer) return ctcdec_state_create(cfg, device, state);
   HostScorer *sc = static_cast<HostScorer *>(scorer);
   if (cfg && (int)sc->labels.size() != cfg->vocab_size)
     return fail(CTCDEC_E_INVALID, "scorer was built for %zu labels, decoder has %d", sc->labels.size(), cfg->vocab_size);
-  int rc = ctcdec_state_create(cfg, device, state);
+  int rc = state_create(cfg, device, true, state);
   if (rc) return rc;
   StreamState *st = static_cast<StreamState *>(*state);
   // node 0 (the root): dictionary start state (0) and LM term 0, reference path_trie.cpp:11-30 / :165-174
@@ -1018,7 +1019,6 @@ static int stream_chunk_step(const ctcdec_config &cfg, Plan &pl, void *const *st
   if ((rc = grow_arenas(states, B, clen.data(), s))) return rc;
   HostScorer *const sc = static_cast<StreamState *>(states[0])->sc;
   if (sc && (rc = ensure_dict_on_device(sc, static_cast<StreamState *>(states[0])->device))) return rc;
-  if (sc) pl.L = make_layout(cfg.beam_size, cfg.vocab_size, pl.NP, pl.F, pl.sorted, pl.NT, true);  // + dictionary masks
   const StreamTabLayout L = stream_tab_layout(B);
   for (int b0 = 0; b0 < B; b0 += kTabPerLaunch) {
     StreamTabArgs a;
@@ -1099,7 +1099,7 @@ int ctcdec_decode_stream_host(const float *probs, const int32_t *seq_lens, int B
   StreamState *s0 = static_cast<StreamState *>(states[0]);
   const ctcdec_config cfg = s0->cfg;
   Plan pl;
-  if ((rc = make_plan(&cfg, B, T, &pl))) return rc;
+  if ((rc = make_plan(&cfg, B, T, &pl, s0->sc != nullptr))) return rc;
   const int device = s0->device;
   if (cudaSetDevice(device) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "cudaSetDevice(%d) failed", device);
   if ((rc = check_device())) return rc;
@@ -1343,7 +1343,7 @@ int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const fl
   const auto t_call0 = std::chrono::steady_clock::now();
   HostScorer *sc = static_cast<HostScorer *>(scorer);
   Plan pl;
-  int rc = make_plan(cfg, B, T, &pl);
+  int rc = make_plan(cfg, B, T, &pl, true);
   if (rc) return rc;
   if ((int)sc->labels.size() != cfg->vocab_size) return fail(CTCDEC_E_INVALID, "scorer was built for %zu labels, decoder has %d", sc->labels.size(), cfg->vocab_size);
   if (device < 0 || device >= 64) return fail(CTCDEC_E_INVALID, "device %d out of range", device);
@@ -1356,7 +1356,6 @@ int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const fl
   cudaStream_t s = c.stream;
   const int V = cfg->vocab_size, K = cfg->beam_size;
   if ((rc = ensure_dict_on_device(sc, device))) return rc;
-  pl.L = make_layout(cfg->beam_size, cfg->vocab_size, pl.NP, pl.F, pl.sorted, pl.NT, true);  // + dictionary masks
   const size_t n_probs = (size_t)B * T * V, n_out = (size_t)B * K * T, n_bk = (size_t)B * K;
   int nls = 0, ups = 0;
   exchange_strides(K, exchange_row_len(*sc), &nls, &ups);
@@ -1453,17 +1452,14 @@ int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const fl
               tmax, hst.workers, std::chrono::duration<double>(std::chrono::steady_clock::now() - c0).count() * 1e3,
               hst.hooks, hst.created);
   } else {
-    Plan pl1 = pl;  // one frame per launch: the staged tile is one row
-    pl1.F = 1;
-    pl1.L = make_layout(K, V, pl.NP, 1, pl.sorted, pl.NT, true);
-
+    // one frame per launch (bp.tile_frames = 1, as in persistent mode): the plan's layout, whose tile holds pl.F rows
     std::vector<int> scratch;
     double t_gpu = 0.0, t_hook = 0.0;
     long long n_hook = 0, n_new = 0;
     for (int t = 0; t < std::max(tmax, 1); ++t) {
       const auto c0 = std::chrono::steady_clock::now();
       bp.t0 = t; bp.nframes = 1; bp.fresh = (t == 0) ? 1 : 0;
-      if ((rc = launch_beam(bp, pl1, B, s))) return rc;
+      if ((rc = launch_beam(bp, pl, B, s))) return rc;
       CU(cudaStreamSynchronize(s));
       const auto c1 = std::chrono::steady_clock::now();
       for (int b = 0; b < B; ++b) {

@@ -28,11 +28,31 @@ static inline size_t al256(size_t x) { return (x + 255) / 256 * 256; }
 
 // streaming multiprocessors of the H100 SXM the launch shapes are sized for (one wave = kNumSMs x CTAs per SM)
 constexpr int kNumSMs = 132;
+// dynamic shared memory one CTA can opt into on the H100 (cudaDevAttrMaxSharedMemoryPerBlockOptin)
+constexpr int kMaxSmemPerCTA = 227 * 1024;
+
+// Launch shape of the prune kernel (prune_program.cuh): a 2 KB head, then per warp the sort keys of the vocabulary
+// (sorted mode, P u64) and, for logits, a staging row of the log-softmax; as many warps per CTA (up to 8) as ~200 KB
+// hold.  The plan refuses a vocabulary whose sort keys alone exceed that (make_plan_core).
+struct PruneShape {
+  int wpc;      // warps per CTA, one frame per warp
+  size_t smem;  // dynamic shared memory per CTA, bytes
+};
+static inline PruneShape prune_shape(const Plan &pl, int V, bool logits) {
+  const size_t row_bytes = logits ? (size_t)((V + 3) / 4 * 4) * 4 : 0;
+  const size_t per_warp = (pl.sorted ? (size_t)pl.P * 8 : 0) + row_bytes;
+  int wpc = 8;
+  if (per_warp > 0) wpc = (int)std::max<size_t>(1, std::min<size_t>(8, (200 * 1024 - 2048) / per_warp));
+  return PruneShape{wpc, 2048 + (size_t)wpc * per_warp};
+}
 
 // b_sched: the number of utterances that will be in flight on the device together (>= B when the caller runs
-// several groups of B concurrently); decides between the latency and the throughput shape of the beam kernel
+// several groups of B concurrently); decides between the latency and the throughput shape of the beam kernel.
+// lm: a scorer is attached.  Its beam kernel carries the [KP][WC] dictionary masks as well (make_layout(..., lm =
+// true)), and pl->L is that layout.  It keeps the two-CTAs-per-SM budget at every batch size: a scorer decode spends
+// its frames in the per-frame host handshake, so three CTAs per SM would not make it faster.
 static inline int make_plan_core(const ctcdec_config *cfg, int B, int T, Plan *pl, char *msg, size_t msglen,
-                                 int nt_override = 0, int b_sched = 0) {
+                                 int nt_override = 0, int b_sched = 0, bool lm = false) {
 #define PLAN_FAIL(code, ...) do { snprintf(msg, msglen, __VA_ARGS__); return code; } while (0)
   if (!cfg) PLAN_FAIL(CTCDEC_E_INVALID, "cfg is NULL");
   const int V = cfg->vocab_size, K = cfg->beam_size;
@@ -65,16 +85,17 @@ static inline int make_plan_core(const ctcdec_config *cfg, int B, int T, Plan *p
     // three CTAs per SM
     pl->NT = 128;
     const SmemLayout t = make_layout(K, V, pl->NP, pl->F, pl->sorted, 128, false, 74);
-    if (t.total <= 74 * 1024 && t.seg * 8 * 4 >= 8 * 1024) budget_kb = 74;
+    if (!lm && t.total <= 74 * 1024 && t.seg * 8 * 4 >= 8 * 1024) budget_kb = 74;
   }
   if (nt_override == 128 || nt_override == 160 || nt_override == 192 || nt_override == 256 || nt_override == 512 || nt_override == 1024) pl->NT = nt_override;
   pl->budget_kb = budget_kb;
-  pl->L = make_layout(K, V, pl->NP, pl->F, pl->sorted, pl->NT, false, budget_kb);
-  if (pl->L.total > 227 * 1024)
-    PLAN_FAIL(CTCDEC_E_UNSUPPORTED, "beam_size %d x pruned vocab %d needs %d bytes of shared memory (> 227 KB)", K,
-              pl->n_max, pl->L.total);
+  pl->L = make_layout(K, V, pl->NP, pl->F, pl->sorted, pl->NT, lm, budget_kb);
+  if (pl->L.total > kMaxSmemPerCTA)
+    PLAN_FAIL(CTCDEC_E_UNSUPPORTED,
+              "beam_size %d x pruned vocab %d needs %d bytes of shared memory%s (> %d, the 227 KB a CTA can have)", K,
+              pl->n_max, pl->L.total, lm ? " with a scorer" : "", kMaxSmemPerCTA);
   if (pl->sorted && 2048 + (size_t)P * 8 > 200 * 1024)
-    PLAN_FAIL(CTCDEC_E_UNSUPPORTED, "vocab_size %d too large for the in-shared-memory vocabulary sort", V);
+    PLAN_FAIL(CTCDEC_E_UNSUPPORTED, "vocab_size %d too large for the in-shared-memory vocabulary sort (at most 16384)", V);
   pl->arena_stride = 1 + (long long)K * T;
   pl->state_stride = (state_ints(K) + 63) / 64 * 64;
   size_t o = 0;

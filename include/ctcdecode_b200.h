@@ -54,7 +54,20 @@ extern "C" {
 
 /* Decoder parameters: the arguments of the reference's ctc_beam_search_decoder_batch
  * (ctc_beam_search_decoder.h:63-72) / paddle_beam_decode (binding.cpp:103-120) that shape the search.
- * `num_processes` has no equivalent: the batch is a CUDA grid, one CTA per utterance. */
+ * `num_processes` has no equivalent: the batch is a CUDA grid, one CTA per utterance.
+ *
+ * Accepted shapes: a beam CTA keeps the whole beam and its candidate lists in the 227 KB of shared memory an H100 CTA
+ * can have, so the largest beam falls as the (pruned) vocabulary grows.  Largest beam without a scorer, batches of
+ * up to 264 utterances (tests/test_plan_envelope.py has every vocabulary, mode and batch plan):
+ *   nothing cut (cutoff_top_n >= V): 736 up to V = 29, 672 at V = 64, 544 at 256, 320 at 1024, 128 at 1500, 64 at
+ *     4096; beams 1-32 take V <= 10845, beam 100 V <= 3389, beam 200 V <= 1469;
+ *   top-40 cut (the default) or cutoff_prob < 1: 736 up to V = 29 (704 at V = 29 with cutoff_prob), 576 at 256, 352
+ *     at 1024, 288 at 1500, 128 at 4096, 32 at 16384; beams 1-32 take V <= 16384 (the vocabulary-sort limit), beam
+ *     100 V <= 4896, beam 200 V <= 2048.
+ * With a scorer: nothing cut 704 at V = 29, 512 at 256, 256 at 1024 (V <= 9053 for beams 1-32); top-40 cut 704 at
+ * V = 29, 608 at 256, 480 at 1024.  Every shape outside returns CTCDEC_E_UNSUPPORTED with the reason (the shared memory
+ * the layout needs, or the sort limit), at plan time: nothing is launched.  The hard bounds beam_size <= 4096 and
+ * vocab_size <= 65534 are never reached. */
 typedef struct ctcdec_config {
   int vocab_size;      /* V = len(labels)                                   */
   int beam_size;       /* beam_width                                         */
