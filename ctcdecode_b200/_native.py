@@ -52,6 +52,11 @@ _SIGNATURES = {
     "ctcdec_scorer_reset_params": (ctypes.c_int, [_vp, ctypes.c_double, ctypes.c_double]),
     "ctcdec_decode_batch_lm_host": (ctypes.c_int, [ctypes.POINTER(Config), _vp, _vp, _vp, ctypes.c_int, ctypes.c_int,
                                                    _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int]),
+    "ctcdec_lm_workspace_bytes": (ctypes.c_int, [ctypes.POINTER(Config), _vp, ctypes.c_int, ctypes.c_int,
+                                                 ctypes.POINTER(ctypes.c_size_t)]),
+    "ctcdec_decode_batch_lm_device": (ctypes.c_int, [ctypes.POINTER(Config), _vp, _vp, ctypes.c_int, _vp, ctypes.c_int,
+                                                     ctypes.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                                     ctypes.c_size_t, _vp]),
     "ctcdec_state_create": (ctypes.c_int, [ctypes.POINTER(Config), ctypes.c_int, ctypes.POINTER(_vp)]),
     "ctcdec_state_create_lm": (ctypes.c_int, [ctypes.POINTER(Config), _vp, ctypes.c_int, ctypes.POINTER(_vp)]),
     "ctcdec_state_destroy": (ctypes.c_int, [_vp]),

@@ -342,6 +342,7 @@ struct DevCache {
   size_t cap[12] = {};
   void *pin[6] = {};  // pinned host staging (scorer path: new-node lists, LM updates; [4]: n_results / flags)
   size_t pcap[6] = {};
+  cudaEvent_t beam_ev = nullptr;  // scorer path: recorded just before the persistent beam launch
 };
 static DevCache g_cache[64];
 static std::mutex g_mu[64];  // one per device: threads driving different GPUs from one process do not serialise
@@ -1336,55 +1337,44 @@ int ctcdec_scorer_reset_params(void *scorer, double alpha, double beta) {
   return CTCDEC_OK;
 }
 
-int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const float *probs, const int32_t *seq_lens,
-                                int B, int T, int32_t *tokens, int32_t *timesteps, float *scores, int32_t *lens,
-                                int32_t *n_results, int32_t *flags, int device) {
-  if (!scorer) return fail(CTCDEC_E_INVALID, "scorer is NULL");
-  const auto t_call0 = std::chrono::steady_clock::now();
-  HostScorer *sc = static_cast<HostScorer *>(scorer);
-  Plan pl;
-  int rc = make_plan(cfg, B, T, &pl, true);
-  if (rc) return rc;
-  if ((int)sc->labels.size() != cfg->vocab_size) return fail(CTCDEC_E_INVALID, "scorer was built for %zu labels, decoder has %d", sc->labels.size(), cfg->vocab_size);
-  if (device < 0 || device >= 64) return fail(CTCDEC_E_INVALID, "device %d out of range", device);
-  if (cudaSetDevice(device) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "cudaSetDevice(%d) failed (this library has no CPU fallback)", device);
-  if ((rc = check_device())) return rc;
-  if (B == 0) return CTCDEC_OK;
-  std::lock_guard<std::mutex> lock(g_mu[device]);
-  DevCache &c = g_cache[device];
-  if (!c.stream) CU(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
-  cudaStream_t s = c.stream;
+// character-based model: the device keeps a row of V LM terms per trie node, batch x (1 + beam x frames) x V floats
+static int lm_row_bytes(const HostScorer *sc, const Plan &pl, int B, size_t *bytes) {
+  *bytes = sc->is_character_based ? (size_t)B * pl.arena_stride * sc->labels.size() * 4 : 0;
+  if (*bytes > ((size_t)64 << 30))
+    return fail(CTCDEC_E_UNSUPPORTED, "character-based model: %zu bytes of per-node rows (batch x (1 + beam x frames) x labels x 4)", *bytes);
+  return CTCDEC_OK;
+}
+
+// Device buffers of one offline scorer decode: the library's own (ctcdec_decode_batch_lm_host, per-device cache) or
+// the caller's outputs and workspace (ctcdec_decode_batch_lm_device).
+struct LmBuffers {
+  PruneInput in;                 // the [B, T, V] input rows
+  const int *seq_lens;           // device copy of seq_lens, or NULL
+  unsigned char *ws;             // the plan's regions (256-byte aligned)
+  float *lm_arena;               // [B][arena_stride] LM term of each trie node
+  int *dstate;                   // [B][arena_stride] dictionary state of each trie node
+  float *lm_row;                 // character-based model: [B][arena_stride][V] rows of LM terms, else NULL
+  int32_t *tokens, *timesteps;   // [B, K, T]
+  float *scores;                 // [B, K] (the raw prefix scores: the caller rescores them with lm_rescore_batch)
+  int32_t *lens, *n_results, *flags;
+};
+
+// One offline scorer decode from the point where the input is on the device, enqueued on s; shared by both scorer
+// entry points, which stage around it (ctcdec_decode_batch_lm_host) or not (ctcdec_decode_batch_lm_device).  Uploads
+// the dictionary, prepares the pinned exchange blocks of `c`, runs the prune scan, the beam kernel (persistent with
+// the per-frame host handshake, or one launch per frame with CTCDEC_LM_PER_FRAME) and enqueues the finalize kernel.
+// seq_lens: the host array (the handshake serves need[b] frames of utterance b).  The caller holds g_mu[device].
+static int lm_batch_step(const ctcdec_config *cfg, const Plan &pl, HostScorer *sc, DevCache &c, int device,
+                         const int32_t *seq_lens, int B, int T, const LmBuffers &io, cudaStream_t s) {
   const int V = cfg->vocab_size, K = cfg->beam_size;
-  if ((rc = ensure_dict_on_device(sc, device))) return rc;
-  const size_t n_probs = (size_t)B * T * V, n_out = (size_t)B * K * T, n_bk = (size_t)B * K;
+  int rc = ensure_dict_on_device(sc, device);
+  if (rc) return rc;
   int nls = 0, ups = 0;
   exchange_strides(K, exchange_row_len(*sc), &nls, &ups);
-  const size_t lm_bytes = al256((size_t)B * pl.arena_stride * 4) * 2;
   const bool lm_char = sc->is_character_based != 0;
-  const size_t row_bytes = lm_char ? (size_t)B * pl.arena_stride * (size_t)V * 4 : 0;  // a row of V terms per node
-  if (row_bytes > ((size_t)64 << 30))
-    return fail(CTCDEC_E_UNSUPPORTED, "character-based model: %zu bytes of per-node rows (batch x (1 + beam x frames) x labels x 4)", row_bytes);
-  if ((rc = ensure(c, 0, n_probs * 4 + 256))) return rc;
-  if ((rc = ensure(c, 1, (size_t)B * 4 + 256))) return rc;
-  if ((rc = ensure(c, 2, n_out * 4 + 256))) return rc;
-  if ((rc = ensure(c, 3, n_out * 4 + 256))) return rc;
-  if ((rc = ensure(c, 4, n_bk * 4 * 2 + (size_t)B * 8 + 1024))) return rc;
-  if ((rc = ensure(c, 5, pl.total + 512))) return rc;
-  if ((rc = ensure(c, 7, lm_bytes + 512))) return rc;
-  if (lm_char && (rc = ensure(c, 8, row_bytes + 256))) return rc;
   if ((rc = ensure_pinned(c, 0, (size_t)B * nls * 4))) return rc;
   if ((rc = ensure_pinned(c, 1, (size_t)B * ups * 4))) return rc;
   if ((rc = ensure_pinned(c, 2, 256))) return rc;
-  float *d_probs = (float *)c.buf[0];
-  int *d_lens_in = seq_lens ? (int *)c.buf[1] : nullptr;
-  int *d_tok = (int *)c.buf[2], *d_ts = (int *)c.buf[3];
-  float *d_scores = (float *)c.buf[4];
-  int *d_lens = (int *)((char *)c.buf[4] + al256(n_bk * 4));
-  int *d_nres = (int *)((char *)d_lens + al256(n_bk * 4));
-  int *d_flags = d_nres + B;
-  unsigned char *lmb = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(c.buf[7]) + 255) / 256 * 256);
-  float *d_lm_arena = (float *)lmb;
-  int *d_dstate = (int *)(lmb + al256((size_t)B * pl.arena_stride * 4));
   int *h_newlist = (int *)c.pin[0], *h_upd = (int *)c.pin[1], *hs_abort = (int *)c.pin[2];
   for (int b = 0; b < B; ++b) { memset(h_newlist + (size_t)b * nls, 0, 16); memset(h_upd + (size_t)b * ups, 0, 8); }
   if (lm_char) {  // the root's row of LM terms: the first entry every CTA picks up before frame 0
@@ -1394,27 +1384,24 @@ int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const fl
   }
   *hs_abort = 0;
 
-  if (n_probs) CU(cudaMemcpyAsync(d_probs, probs, n_probs * 4, cudaMemcpyHostToDevice, s));
-  if (seq_lens) CU(cudaMemcpyAsync(d_lens_in, seq_lens, (size_t)B * 4, cudaMemcpyHostToDevice, s));
-  CU(cudaMemsetAsync(d_flags, 0, (size_t)B * 4, s));
-  unsigned char *ws = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(c.buf[5]) + 255) / 256 * 256);
-  float *lp = reinterpret_cast<float *>(ws + pl.off_lp);
-  uint16_t *idx = pl.sorted ? reinterpret_cast<uint16_t *>(ws + pl.off_idx) : nullptr;
-  if ((rc = launch_prune(cfg, pl, PruneInput{d_probs, IN_F32, nullptr, true}, d_lens_in, B, T, lp, idx, d_flags, s))) return rc;
+  CU(cudaMemsetAsync(io.flags, 0, (size_t)B * 4, s));
+  float *lp = reinterpret_cast<float *>(io.ws + pl.off_lp);
+  uint16_t *idx = pl.sorted ? reinterpret_cast<uint16_t *>(io.ws + pl.off_idx) : nullptr;
+  if ((rc = launch_prune(cfg, pl, io.in, io.seq_lens, B, T, lp, idx, io.flags, s))) return rc;
 
   BeamParams bp;
   memset(&bp, 0, sizeof(bp));
-  bp.lp = lp; bp.idx = idx; bp.seq_lens = d_lens_in; bp.T = T; bp.V = V; bp.NP = pl.NP; bp.K = K;
+  bp.lp = lp; bp.idx = idx; bp.seq_lens = io.seq_lens; bp.T = T; bp.V = V; bp.NP = pl.NP; bp.K = K;
   bp.blank = cfg->blank_id; bp.tile_frames = 1;
-  bp.arena = reinterpret_cast<Node *>(ws + pl.off_arena); bp.arena_stride = pl.arena_stride;
-  bp.state = reinterpret_cast<int *>(ws + pl.off_state); bp.state_stride = pl.state_stride;
+  bp.arena = reinterpret_cast<Node *>(io.ws + pl.off_arena); bp.arena_stride = pl.arena_stride;
+  bp.state = reinterpret_cast<int *>(io.ws + pl.off_state); bp.state_stride = pl.state_stride;
   bp.arena_cap = (int)pl.arena_stride;
-  bp.out_tokens = d_tok; bp.out_timesteps = d_ts; bp.out_scores = d_scores; bp.out_lens = d_lens;
-  bp.n_results = d_nres; bp.out_T = T; bp.flags = d_flags;
+  bp.out_tokens = io.tokens; bp.out_timesteps = io.timesteps; bp.out_scores = io.scores; bp.out_lens = io.lens;
+  bp.n_results = io.n_results; bp.out_T = T; bp.flags = io.flags;
   bp.force_fallback = getenv("CTCDEC_FORCE_FALLBACK") ? 1 : 0;
   bp.dict_next = sc->d_next; bp.dict_mask = sc->d_mask; bp.dict_wc = sc->dict.wc; bp.dict_start = sc->dict.start;
-  bp.space_id = sc->space_id; bp.beta = sc->beta; bp.lm_arena = d_lm_arena; bp.dstate_arena = d_dstate;
-  bp.lm_char = lm_char ? 1 : 0; bp.lm_row = lm_char ? (float *)c.buf[8] : nullptr;
+  bp.space_id = sc->space_id; bp.beta = sc->beta; bp.lm_arena = io.lm_arena; bp.dstate_arena = io.dstate;
+  bp.lm_char = lm_char ? 1 : 0; bp.lm_row = lm_char ? io.lm_row : nullptr;
   bp.timing = g_prof.timing;
   // The per-frame exchange with the host goes through pinned, device-mapped host memory (unified addressing):
   // the kernel reads the few LM updates and writes the new-node list straight over PCIe, so a frame costs one
@@ -1437,7 +1424,16 @@ int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const fl
     bp.lm_persistent = 1; bp.hs_abort = hs_abort;
     bp.t0 = 0; bp.nframes = 0; bp.fresh = 1;
     const auto c0 = std::chrono::steady_clock::now();
+    if (!c.beam_ev) CU(cudaEventCreateWithFlags(&c.beam_ev, cudaEventDisableTiming));
+    CU(cudaEventRecord(c.beam_ev, s));
     if ((rc = launch_beam(bp, pl, B, s))) return rc;
+    // the handshake gives up after 8 s without progress: start its clock once the work queued on s before the beam
+    // kernel (the caller's, on a stream of the caller's) has finished
+    const cudaError_t ew = cudaEventSynchronize(c.beam_ev);
+    if (ew != cudaSuccess) {
+      reinterpret_cast<std::atomic<int> *>(hs_abort)->store(1, std::memory_order_release);
+      return fail(CTCDEC_E_CUDA, "work queued before the beam kernel (scorer path): %s", cudaGetErrorString(ew));
+    }
     std::vector<TrieMirror *> mirrors(B);
     std::vector<int> answers(B);
     for (int b = 0; b < B; ++b) { mirrors[b] = &mirror[b]; answers[b] = std::max(0, need[b] - 1); }
@@ -1475,8 +1471,62 @@ int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const fl
       fprintf(stderr, "[ctcdec lm] frames %d: launch+copy+sync %.1f ms, host mirror+hooks %.1f ms (%lld hook calls, %lld new nodes)\n",
               tmax, t_gpu * 1e3, t_hook * 1e3, n_hook, n_new);
   }
+  return launch_finalize(bp, B, s);
+}
+
+int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const float *probs, const int32_t *seq_lens,
+                                int B, int T, int32_t *tokens, int32_t *timesteps, float *scores, int32_t *lens,
+                                int32_t *n_results, int32_t *flags, int device) {
+  if (!scorer) return fail(CTCDEC_E_INVALID, "scorer is NULL");
+  const auto t_call0 = std::chrono::steady_clock::now();
+  HostScorer *sc = static_cast<HostScorer *>(scorer);
+  Plan pl;
+  int rc = make_plan(cfg, B, T, &pl, true);
+  if (rc) return rc;
+  if ((int)sc->labels.size() != cfg->vocab_size) return fail(CTCDEC_E_INVALID, "scorer was built for %zu labels, decoder has %d", sc->labels.size(), cfg->vocab_size);
+  if (device < 0 || device >= 64) return fail(CTCDEC_E_INVALID, "device %d out of range", device);
+  if (cudaSetDevice(device) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "cudaSetDevice(%d) failed (this library has no CPU fallback)", device);
+  if ((rc = check_device())) return rc;
+  if (B == 0) return CTCDEC_OK;
+  std::lock_guard<std::mutex> lock(g_mu[device]);
+  DevCache &c = g_cache[device];
+  if (!c.stream) CU(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
+  cudaStream_t s = c.stream;
+  const int V = cfg->vocab_size, K = cfg->beam_size;
+  const size_t n_probs = (size_t)B * T * V, n_out = (size_t)B * K * T, n_bk = (size_t)B * K;
+  const size_t lm_bytes = al256((size_t)B * pl.arena_stride * 4) * 2;
+  size_t row_bytes = 0;
+  if ((rc = lm_row_bytes(sc, pl, B, &row_bytes))) return rc;
+  if ((rc = ensure(c, 0, n_probs * 4 + 256))) return rc;
+  if ((rc = ensure(c, 1, (size_t)B * 4 + 256))) return rc;
+  if ((rc = ensure(c, 2, n_out * 4 + 256))) return rc;
+  if ((rc = ensure(c, 3, n_out * 4 + 256))) return rc;
+  if ((rc = ensure(c, 4, n_bk * 4 * 2 + (size_t)B * 8 + 1024))) return rc;
+  if ((rc = ensure(c, 5, pl.total + 512))) return rc;
+  if ((rc = ensure(c, 7, lm_bytes + 512))) return rc;
+  if (row_bytes && (rc = ensure(c, 8, row_bytes + 256))) return rc;
+  float *d_probs = (float *)c.buf[0];
+  int *d_lens_in = seq_lens ? (int *)c.buf[1] : nullptr;
+  int *d_tok = (int *)c.buf[2], *d_ts = (int *)c.buf[3];
+  float *d_scores = (float *)c.buf[4];
+  int *d_lens = (int *)((char *)c.buf[4] + al256(n_bk * 4));
+  int *d_nres = (int *)((char *)d_lens + al256(n_bk * 4));
+  int *d_flags = d_nres + B;
+  unsigned char *lmb = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(c.buf[7]) + 255) / 256 * 256);
+  if (n_probs) CU(cudaMemcpyAsync(d_probs, probs, n_probs * 4, cudaMemcpyHostToDevice, s));
+  if (seq_lens) CU(cudaMemcpyAsync(d_lens_in, seq_lens, (size_t)B * 4, cudaMemcpyHostToDevice, s));
+  LmBuffers io;
+  io.in = PruneInput{d_probs, IN_F32, nullptr, true};
+  io.seq_lens = d_lens_in;
+  io.ws = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(c.buf[5]) + 255) / 256 * 256);
+  io.lm_arena = (float *)lmb;
+  io.dstate = (int *)(lmb + al256((size_t)B * pl.arena_stride * 4));
+  io.lm_row = row_bytes ? (float *)c.buf[8] : nullptr;
+  io.tokens = d_tok; io.timesteps = d_ts; io.scores = d_scores; io.lens = d_lens; io.n_results = d_nres;
+  io.flags = d_flags;
+  if ((rc = lm_batch_step(cfg, pl, sc, c, device, seq_lens, B, T, io, s))) return rc;
+  const bool lm_timing = getenv("CTCDEC_LM_TIMING") != nullptr;
   const auto t_fin0 = std::chrono::steady_clock::now();
-  if ((rc = launch_finalize(bp, B, s))) return rc;
   std::unique_ptr<int[]> h_nres(new int[(size_t)B * 2]);
   std::unique_ptr<float[]> h_scores(new float[n_bk]);
   std::unique_ptr<int[]> h_lens(new int[n_bk]);
@@ -1519,6 +1569,123 @@ int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const fl
   if (n_results) memcpy(n_results, h_nres.get(), (size_t)B * 4);
   if (flags) memcpy(flags, h_nres.get() + B, (size_t)B * 4);
   return check_error_flags(h_nres.get() + B, B);
+}
+
+// Device scratch of ctcdec_decode_batch_lm_device: the plan's regions, then the per-node LM terms and dictionary
+// states, for a character-based model the per-node rows of LM terms, and the device copy of seq_lens.
+struct LmWorkspace { size_t lm_arena, dstate, rows, lens, total; };
+static int lm_workspace(const HostScorer *sc, const Plan &pl, int B, LmWorkspace *w) {
+  size_t row_bytes = 0;
+  const int rc = lm_row_bytes(sc, pl, B, &row_bytes);
+  if (rc) return rc;
+  const size_t node_bytes = al256((size_t)B * pl.arena_stride * 4);
+  w->lm_arena = pl.total;
+  w->dstate = w->lm_arena + node_bytes;
+  w->rows = w->dstate + node_bytes;
+  w->lens = w->rows + al256(row_bytes);
+  w->total = w->lens + al256((size_t)B * 4);
+  return CTCDEC_OK;
+}
+
+// the checks both scorer device functions make before anything else: the scorer, the plan with a scorer, the labels
+static int lm_device_plan(const ctcdec_config *cfg, const void *scorer, int B, int T, Plan *pl, LmWorkspace *w) {
+  if (!scorer) return fail(CTCDEC_E_INVALID, "scorer is NULL");
+  const HostScorer *sc = static_cast<const HostScorer *>(scorer);
+  int rc = make_plan(cfg, B, T, pl, true);
+  if (rc) return rc;
+  if ((int)sc->labels.size() != cfg->vocab_size)
+    return fail(CTCDEC_E_INVALID, "scorer was built for %zu labels, decoder has %d", sc->labels.size(), cfg->vocab_size);
+  return lm_workspace(sc, *pl, B, w);
+}
+
+int ctcdec_lm_workspace_bytes(const ctcdec_config *cfg, const void *scorer, int B, int T, size_t *bytes) {
+  Plan pl;
+  LmWorkspace w;
+  const int rc = lm_device_plan(cfg, scorer, B, T, &pl, &w);
+  if (rc) return rc;
+  if (!bytes) return fail(CTCDEC_E_INVALID, "bytes is NULL");
+  *bytes = w.total + 256;
+  return CTCDEC_OK;
+}
+
+int ctcdec_decode_batch_lm_device(const ctcdec_config *cfg, void *scorer, const void *input, int dtype,
+                                  const int32_t *seq_lens, int B, int T, int32_t *tokens, int32_t *timesteps,
+                                  float *scores, int32_t *lens, int32_t *n_results, int32_t *flags,
+                                  float *log_probs_out, void *workspace, size_t workspace_bytes, void *stream) {
+  if (!scorer) return fail(CTCDEC_E_INVALID, "scorer is NULL");
+  if (dtype != -1 && dtype != CTCDEC_DTYPE_F32 && dtype != CTCDEC_DTYPE_F16 && dtype != CTCDEC_DTYPE_BF16)
+    return fail(CTCDEC_E_INVALID, "dtype %d is not -1 (probabilities) or one of CTCDEC_DTYPE_F32 / F16 / BF16", dtype);
+  const int kind = dtype == -1 ? IN_F32 : dtype == CTCDEC_DTYPE_F32 ? IN_LOGITS_F32
+                 : dtype == CTCDEC_DTYPE_F16 ? IN_LOGITS_F16 : IN_LOGITS_BF16;
+  Plan pl;
+  LmWorkspace w;
+  int rc = lm_device_plan(cfg, scorer, B, T, &pl, &w);
+  if (rc) return rc;
+  HostScorer *sc = static_cast<HostScorer *>(scorer);
+  if (B > 0 && (!n_results || !flags)) return fail(CTCDEC_E_INVALID, "n_results and flags device buffers are required");
+  if (B > 0 && (!scores || !lens || (T > 0 && (!input || !tokens || !timesteps))))
+    return fail(CTCDEC_E_INVALID, "the input or an output pointer is NULL");
+  if ((rc = check_device())) return rc;
+  int device = 0;
+  CU(cudaGetDevice(&device));
+  if (device >= 64) return fail(CTCDEC_E_INVALID, "device %d out of range", device);
+  if (B == 0) return CTCDEC_OK;
+  const size_t need_bytes = w.total + 256;
+  if (!workspace || workspace_bytes < need_bytes)
+    return fail(CTCDEC_E_WORKSPACE, "workspace of %zu bytes given, %zu needed", workspace_bytes, need_bytes);
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  // the host answers the beam kernel's per-frame handshake while the call runs: a captured graph could not replay that
+  cudaStreamCaptureStatus capturing = cudaStreamCaptureStatusNone;
+  CU(cudaStreamIsCapturing(s, &capturing));
+  if (capturing != cudaStreamCaptureStatusNone)
+    return fail(CTCDEC_E_UNSUPPORTED, "the scorer path cannot be captured into a CUDA graph (the host answers the beam "
+                "kernel's per-frame handshake during the call)");
+  const int K = cfg->beam_size;
+  const size_t n_bk = (size_t)B * K;
+  std::lock_guard<std::mutex> lock(g_mu[device]);
+  DevCache &c = g_cache[device];
+  unsigned char *ws = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(workspace) + 255) / 256 * 256);
+  int *d_lens_in = seq_lens ? reinterpret_cast<int *>(ws + w.lens) : nullptr;
+  if (seq_lens) CU(cudaMemcpyAsync(d_lens_in, seq_lens, (size_t)B * 4, cudaMemcpyHostToDevice, s));
+  LmBuffers io;
+  io.in = PruneInput{input, kind, kind == IN_F32 ? nullptr : log_probs_out, true};
+  io.seq_lens = d_lens_in;
+  io.ws = ws;
+  io.lm_arena = reinterpret_cast<float *>(ws + w.lm_arena);
+  io.dstate = reinterpret_cast<int *>(ws + w.dstate);
+  io.lm_row = sc->is_character_based ? reinterpret_cast<float *>(ws + w.rows) : nullptr;
+  io.tokens = tokens; io.timesteps = timesteps; io.scores = scores; io.lens = lens; io.n_results = n_results;
+  io.flags = flags;
+  if ((rc = lm_batch_step(cfg, pl, sc, c, device, seq_lens, B, T, io, s))) return rc;
+  // Read-out: the finalize kernel wrote the rows in place; the reported scores are the reference's approx_ctc, which
+  // needs the sentence hook on each row's labels, so columns [0, max_len) of the rows come to pinned staging
+  std::unique_ptr<int[]> h_nres(new int[(size_t)B * 2]);
+  int *const h_flags = h_nres.get() + B;
+  std::unique_ptr<float[]> h_scores(new float[n_bk]);
+  std::unique_ptr<int[]> h_lens(new int[n_bk]);
+  CU(cudaMemcpyAsync(h_scores.get(), scores, n_bk * 4, cudaMemcpyDeviceToHost, s));
+  CU(cudaMemcpyAsync(h_lens.get(), lens, n_bk * 4, cudaMemcpyDeviceToHost, s));
+  CU(cudaMemcpyAsync(h_nres.get(), n_results, (size_t)B * 4, cudaMemcpyDeviceToHost, s));
+  CU(cudaMemcpyAsync(h_flags, flags, (size_t)B * 4, cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s));
+  int max_len = 0;
+  for (int b = 0; b < B; ++b)
+    for (int p = 0; p < h_nres[b] && p < K; ++p) max_len = std::max(max_len, h_lens[(size_t)b * K + p]);
+  if (max_len > T) max_len = T;
+  static const int32_t no_rows = 0;
+  const int32_t *stage_tok = &no_rows;
+  if (max_len > 0) {
+    if ((rc = ensure_pinned(c, 5, n_bk * (size_t)max_len * 4))) return rc;
+    int32_t *const st = static_cast<int32_t *>(c.pin[5]);
+    CU(cudaMemcpy2DAsync(st, (size_t)max_len * 4, tokens, (size_t)T * 4, (size_t)max_len * 4, n_bk, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    stage_tok = st;
+  }
+  lm_rescore_batch(*sc, B, K, max_len, h_nres.get(), stage_tok, h_lens.get(), h_scores.get());
+  // (rows p >= n_results[b] go back as they were read: the caller's values, unchanged)
+  CU(cudaMemcpyAsync(scores, h_scores.get(), n_bk * 4, cudaMemcpyHostToDevice, s));
+  CU(cudaStreamSynchronize(s));
+  return check_error_flags(h_flags, B);
 }
 
 int ctcdec_rows_to_host(const int32_t *d_tokens, const int32_t *d_timesteps, long long rows, int row_stride, int max_len,

@@ -7,14 +7,17 @@ include/ctcdecode_b200.h into the sm_90a kernels.  There is no CPU fallback: wit
 without an H100 the calls raise.
 
 Differences from the reference, all additive:
-  * ``probs`` may live on the GPU; it is then decoded in place (the reference does ``probs.cpu()`` first,
-    __init__.py:77).  Results are CPU tensors like the reference's unless ``device_outputs=True``.
+  * ``probs`` may live on the GPU; it is then decoded in place, with or without a scorer (the reference does
+    ``probs.cpu()`` first, __init__.py:77).  Results are CPU tensors like the reference's unless
+    ``device_outputs=True``.  ``decode_logits`` takes the acoustic model's raw logits instead, also with a scorer.
   * ``num_processes`` is accepted and ignored: the batch is a CUDA grid (one CTA per utterance).
   * ``decoder.last_flags`` / ``decoder.last_n_results`` expose the per-utterance tie flags and beam counts
     of the last call (the reference has no equivalent; see include/ctcdecode_b200.h).
   * ``model_path`` (word-based KenLM models): the language model stays on the host behind a hook; the real Scorer
     comes from a provider library (``scorer_provider=`` / CTCDECODE_B200_SCORER_PROVIDER, see scorer.py and
-    INTEGRATION.md; providers/ builds one from the reference's own Scorer + KenLM).  The online decoder takes a
+    INTEGRATION.md; providers/ builds one from the reference's own Scorer + KenLM).  CUDA probabilities and logits
+    stay on the GPU with a scorer too (ctcdec_decode_batch_lm_device); that call returns when the results are in place,
+    because the host answers the beam kernel's per-frame LM handshake while it runs.  The online decoder takes a
     scorer too (device-resident states, one persistent launch per chunk).  Character-based models are detected like
     the reference does (every word of the model is one UTF-8 character) and decoded without a dictionary.
   * the [batch, beam, T] result tensors are PAGE-LOCKED CPU tensors (torch's caching host allocator, so a decode loop
@@ -133,7 +136,7 @@ class CTCBeamDecoder(_Base):
             raise ValueError("probs has %d labels, decoder was built with %d" % (V, self._num_labels))
         cfg = _cfg(self)
         K = self._beam_width
-        if probs.is_cuda and self._scorer is None:
+        if probs.is_cuda:
             return self._decode_device(lib, cfg, probs, seq_lens, B, T, K)
         dev_index = self._device_index(probs)
         probs = probs.cpu().float().contiguous()
@@ -171,10 +174,8 @@ class CTCBeamDecoder(_Base):
         (README.md:54-57): the scan kernel computes each frame's float32 log-softmax on the fly and decodes as with
         log_probs_input=True.  Returns the usual four tensors, plus -- with return_log_probs -- the float32
         log-softmax the decode used (feeding that to the reference with log_probs_input=True reproduces the result
-        bit for bit)."""
+        bit for bit).  With a scorer the language model is applied as in decode (the call then waits for the device)."""
         lib = _native.load()
-        if self._scorer is not None:
-            raise NotImplementedError("ctcdecode_b200: decode_logits with a scorer is not built")
         if logits.dim() != 3 or not logits.is_cuda:
             raise ValueError("logits must be a CUDA tensor [batch, time, labels]")
         dtypes = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
@@ -217,12 +218,17 @@ class CTCBeamDecoder(_Base):
 
     def _decode_device(self, lib, cfg, probs, seq_lens, B, T, K, logits_dtype=None, lsm_out=None):
         dev = probs.device
+        scorer = self._scorer.handle if self._scorer is not None else None
         if logits_dtype is None:
             probs = probs.float().contiguous()
         if seq_lens is not None:
-            seq_lens = seq_lens.to(device=dev, dtype=torch.int32).contiguous()
+            # (the scorer path answers every utterance's per-frame handshake on the host: its lengths stay there)
+            seq_lens = seq_lens.to(device="cpu" if scorer else dev, dtype=torch.int32).contiguous()
         nbytes = ctypes.c_size_t(0)
-        _native.check(lib.ctcdec_workspace_bytes(ctypes.byref(cfg), B, T, ctypes.byref(nbytes)))
+        if scorer:
+            _native.check(lib.ctcdec_lm_workspace_bytes(ctypes.byref(cfg), scorer, B, T, ctypes.byref(nbytes)))
+        else:
+            _native.check(lib.ctcdec_workspace_bytes(ctypes.byref(cfg), B, T, ctypes.byref(nbytes)))
         if self._ws is None or self._ws.numel() < nbytes.value or self._ws.device != dev:
             self._ws = None
             self._ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
@@ -234,7 +240,14 @@ class CTCBeamDecoder(_Base):
         flags = torch.zeros(B, dtype=torch.int32, device=dev)
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev).cuda_stream
-            if logits_dtype is None:
+            if scorer:  # (returns when the results are in place: the host serves the LM during the call)
+                _native.check(lib.ctcdec_decode_batch_lm_device(
+                    ctypes.byref(cfg), scorer, probs.data_ptr(), -1 if logits_dtype is None else logits_dtype,
+                    seq_lens.data_ptr() if seq_lens is not None else None, B, T, output.data_ptr(),
+                    timesteps.data_ptr(), scores.data_ptr(), out_seq_len.data_ptr(), n_results.data_ptr(),
+                    flags.data_ptr(), lsm_out.data_ptr() if lsm_out is not None else None, self._ws.data_ptr(),
+                    self._ws.numel(), stream))
+            elif logits_dtype is None:
                 _native.check(lib.ctcdec_decode_batch_device(
                     ctypes.byref(cfg), probs.data_ptr(), seq_lens.data_ptr() if seq_lens is not None else None, B, T,
                     output.data_ptr(), timesteps.data_ptr(), scores.data_ptr(), out_seq_len.data_ptr(),

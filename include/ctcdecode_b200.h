@@ -25,7 +25,8 @@
  *       flags      int32   [B]   CTCDEC_FLAG_* bits; the TIE bits mark utterances where the
  *                                reference's own result is unspecified (equal score AND equal last
  *                                character straddling a cut -- std::nth_element / std::sort internals)
- *   - "device" entry points take device pointers and a CUDA stream and never synchronise; "host"
+ *   - "device" entry points take device pointers and a CUDA stream and never synchronise (except the scorer
+ *     path's ctcdec_decode_batch_lm_device, whose language model is answered by the host during the call); "host"
  *     entry points take host pointers, stage through pinned memory and return when results are in
  *     the caller's buffers (what the reference's CPU-tensor API looks like to its caller).
  */
@@ -186,6 +187,34 @@ int ctcdec_scorer_reset_params(void *scorer, double alpha, double beta);
 int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const float *probs, const int32_t *seq_lens,
                                 int B, int T, int32_t *tokens, int32_t *timesteps, float *scores, int32_t *lens,
                                 int32_t *n_results, int32_t *flags, int device);
+
+/* Bytes of device scratch ctcdec_decode_batch_lm_device needs for a [B, T, V] batch with this scorer: the regions of
+ * ctcdec_workspace_bytes' plan, then the LM term and the dictionary state of every trie node (2 x batch x (1 + beam x
+ * T) x 4 bytes, each 256-byte aligned), for a character-based model the per-node rows of LM terms (batch x (1 + beam x
+ * T) x V x 4, CTCDEC_E_UNSUPPORTED beyond 64 GiB), and a device copy of seq_lens.  Checks the scorer and the shape
+ * like the decode does: the same refusals, no device needed. */
+int ctcdec_lm_workspace_bytes(const ctcdec_config *cfg, const void *scorer, int B, int T, size_t *bytes);
+
+/* ctcdec_decode_batch_lm_host with the input and the results on the DEVICE (the current device), in the caller's
+ * workspace.  Extension: the reference's scorer path decodes CPU tensors only.
+ *   input      [B, T, V] device buffer.  dtype -1: float32 probabilities, or log-probabilities if cfg->log_input;
+ *              CTCDEC_DTYPE_F32 / F16 / BF16: raw logits, log-softmaxed per frame by the scan kernel as in
+ *              ctcdec_decode_batch_device_logits (cfg->log_input is ignored; log_probs_out, optional, receives the
+ *              float32 log-softmax rows the decode used).
+ *   seq_lens   HOST int32 [B] or NULL: the host answers each utterance's per-frame handshake and must know its length.
+ *   tokens / timesteps [B, beam, T], scores / lens [B, beam], n_results / flags [B]: device buffers, n_results and
+ *              flags required (B > 0).  Rows p >= n_results[b] are left untouched.  scores hold the reported (approx_ctc)
+ *              scores, as with the host entry.
+ * BLOCKING, unlike the other device entry points: the host answers the beam kernel's per-frame handshake during the
+ * call, which returns when every output is in place.  The prune and beam kernels go onto `stream` after the work
+ * already queued there; the handshake's 8 s no-progress limit starts once that work has finished.  A stream that is
+ * being captured into a CUDA graph is refused with CTCDEC_E_UNSUPPORTED before anything is enqueued.  The plan is the
+ * host entry's (the same accepted shapes); CTCDEC_LM_PER_FRAME=1 selects one launch per frame here too.  A set
+ * CTCDEC_FLAG_ERR_ARENA returns CTCDEC_E_INTERNAL, as with the host entry points.  Calls on one device serialise. */
+int ctcdec_decode_batch_lm_device(const ctcdec_config *cfg, void *scorer, const void *input, int dtype,
+                                  const int32_t *seq_lens, int B, int T, int32_t *tokens, int32_t *timesteps,
+                                  float *scores, int32_t *lens, int32_t *n_results, int32_t *flags,
+                                  float *log_probs_out, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ---- streaming (OnlineCTCBeamDecoder) ------------------------------------------------------------- */
 

@@ -1,0 +1,93 @@
+#!/usr/bin/env python
+"""Scorer-path benchmark: BASELINE config 5 ([64 x T=1000 x V=29], beam 100, the reference's test.arpa, alpha 2.0,
+beta 1.0) through CTCBeamDecoder three ways:
+
+  host            CPU probabilities through the host entry point (ctcdec_decode_batch_lm_host)
+  device          CUDA probabilities through the device entry point (ctcdec_decode_batch_lm_device)
+  logits_f16      decode_logits of fp16 logits (the device entry, the log-softmax taken by the scan kernel)
+
+    python tools/lm_device_bench.py [--reps N] [--device I]
+
+Every path is warmed up, then timed N times in alternating rounds with a host clock around the call (each call
+returns synchronised, with CPU results).  Prints one JSON line: per path the median and the spread of the call time
+and utterances/s; whether the host and device paths gave identical outputs; the card and its power limit, read in the
+same run.  Writes nothing to disk.
+"""
+import argparse
+import json
+import os
+import statistics
+import sys
+import time
+
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+from bench import CONFIGS, L29, PROVIDER, TINY_LM, c5_inputs  # noqa: E402
+from ctcdecode_b200 import CTCBeamDecoder  # noqa: E402
+from tools.stream_bench import card_info  # noqa: E402
+
+
+def identical(x, y):
+    """bit for bit: n_results, flags, and per row p < n_results the score bits, the length, tokens and timesteps"""
+    tok_x, sc_x, ts_x, ln_x, nr_x, fl_x = x
+    tok_y, sc_y, ts_y, ln_y, nr_y, fl_y = y
+    if not (torch.equal(nr_x, nr_y) and torch.equal(fl_x, fl_y)):
+        return False
+    for b in range(nr_x.shape[0]):
+        n = int(nr_x[b])
+        if not (torch.equal(sc_x[b, :n].view(torch.int32), sc_y[b, :n].view(torch.int32)) and
+                torch.equal(ln_x[b, :n], ln_y[b, :n])):
+            return False
+        for p in range(n):
+            L = int(ln_x[b, p])
+            if not (torch.equal(tok_x[b, p, :L], tok_y[b, p, :L]) and torch.equal(ts_x[b, p, :L], ts_y[b, p, :L])):
+                return False
+    return True
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--reps", type=int, default=5, help="timed calls per path")
+    ap.add_argument("--device", type=int, default=0)
+    args = ap.parse_args()
+    dev = torch.device("cuda", args.device)
+    torch.cuda.set_device(dev)
+    cfg = CONFIGS["c5"]
+    B, T = cfg["B"], cfg["T"]
+    probs = c5_inputs(B, T, 0)
+    probs_d = probs.to(dev)
+    logits = probs_d.clamp_min(1e-20).log().mul(1.25).half()
+    dec = CTCBeamDecoder(L29, model_path=TINY_LM, alpha=cfg["alpha"], beta=cfg["beta"], beam_width=cfg["beam"],
+                         cutoff_top_n=cfg["cutoff_top_n"], cutoff_prob=cfg["cutoff_prob"], scorer_provider=PROVIDER)
+    paths = {"host": lambda: dec.decode(probs), "device": lambda: dec.decode(probs_d),
+             "logits_f16": lambda: dec.decode_logits(logits)}
+
+    def call(name):
+        t0 = time.perf_counter()
+        res = paths[name]()
+        torch.cuda.synchronize(dev)
+        dt = time.perf_counter() - t0
+        return dt, list(res) + [dec.last_n_results.clone(), dec.last_flags.clone()]
+
+    outs, times = {}, {name: [] for name in paths}
+    for name in paths:
+        for _ in range(2):
+            call(name)  # warm-up: workspace, pinned blocks, dictionary upload, kernel attributes, hook caches
+    for _ in range(args.reps):
+        for name in paths:
+            dt, outs[name] = call(name)
+            times[name].append(dt)
+    legs = {name: {"ms_median": 1e3 * statistics.median(t), "ms_min": 1e3 * min(t), "ms_max": 1e3 * max(t),
+                   "utterances_per_s": B / statistics.median(t), "calls": len(t)} for name, t in times.items()}
+    same = identical(outs["host"], outs["device"])
+    print(json.dumps({"workload": cfg["name"], "card": card_info(args.device), "paths": legs,
+                      "host_device_identical": bool(same),
+                      "note": "host clock around each call, which returns synchronised with CPU results; paths "
+                              "alternate within each round"}), flush=True)
+    assert same, "host and device entry points gave different results"
+
+
+if __name__ == "__main__":
+    main()
