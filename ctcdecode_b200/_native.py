@@ -45,6 +45,10 @@ _SIGNATURES = {
     "ctcdec_scorer_create": (ctypes.c_int, [_vp, ctypes.c_double, ctypes.c_double, ctypes.POINTER(ctypes.c_char_p),
                                             ctypes.c_int, ctypes.POINTER(ctypes.c_char_p), ctypes.c_int, ctypes.c_int,
                                             ctypes.c_int, ctypes.POINTER(_vp)]),
+    "ctcdec_scorer_create_arpa": (ctypes.c_int, [ctypes.c_char_p, ctypes.c_double, ctypes.c_double,
+                                                 ctypes.POINTER(ctypes.c_char_p), ctypes.c_int, ctypes.POINTER(_vp)]),
+    "ctcdec_scorer_cond_log_prob": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.POINTER(ctypes.c_double)]),
+    "ctcdec_scorer_sent_log_prob": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.POINTER(ctypes.c_double)]),
     "ctcdec_scorer_destroy": (ctypes.c_int, [_vp]),
     "ctcdec_scorer_is_character_based": (ctypes.c_int, [_vp]),
     "ctcdec_scorer_max_order": (ctypes.c_int, [_vp]),

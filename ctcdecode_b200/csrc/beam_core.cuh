@@ -34,6 +34,7 @@
 #include <cstdint>
 
 #include "glibc_math.cuh"
+#include "ngram_lm.h"
 
 // CTC_PAR { ... }                 a parallel region over the NT threads of the CTA (variable `tid`)
 // CTC_WARPS { ... CTC_LANES { ... } ... }   a warp-structured region: code directly inside CTC_WARPS is
@@ -278,6 +279,15 @@ struct BeamParams {
   int *hs_abort;                    // [1] mapped host memory: host asks the kernel to stop waiting
   void (*emu_handshake)(void *ctx, int b);  // CPU emulation only: the host side of the handshake, called in place
   void *emu_ctx;
+  // device n-gram scorer (an ARPA scorer, ngram_lm.h): the CTA computes the LM terms of the nodes it creates itself, so
+  // there are no exchange blocks and no handshake (lm_persistent = 0, newlist / lm_upd unused)
+  int lm_dev;
+  double lm_alpha;                  // Scorer::alpha: a term is float(cond_log_prob * alpha), as the host computes it
+  NgramView ngram;                  // the model's tables in device memory
+  const int *word_of_state;         // word-based: [n_states] the word a dictionary state completes with a space
+  const int *label_word;            // character-based: [V] the word id of each label
+  int lm_hist_n;                    // order - 1
+  int *lm_hist;                     // [B][arena_stride][order - 1] the node's last order - 1 LM word ids, oldest first
 };
 
 // control words: 32 ints in L.ctl

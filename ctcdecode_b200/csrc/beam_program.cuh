@@ -36,6 +36,39 @@
 
 namespace ctc {
 
+// ---- device n-gram scorer (BeamParams::lm_dev): the LM terms of a node, computed by the thread that creates it -----
+// A node keeps the last order - 1 LM word ids of its prefix (oldest first, "<s>"-padded like Scorer::make_ngram).  A
+// child through the space label shifts in the word its parent's dictionary state completes; in a character-based model
+// every child shifts in its character's word id; any other child keeps its parent's history.  The terms are those the
+// host hooks give (lm_host.h lm_after_frame / lm_char_row): float(cond_log_prob * alpha) of history + the node's word
+// (word-based, when a space can follow the node) or of history + each label (character-based, the node's row).
+CTC_FN float lm_dev_term(const BeamParams &p, int *ids, int word) {
+  ids[p.lm_hist_n] = word;
+  return (float)(ngram_cond_ids(p.ngram, ids, p.lm_hist_n + 1) * p.lm_alpha);
+}
+
+CTC_FN void lm_dev_root_term(const BeamParams &p, float *lm_row, int c) {
+  int ids[kNgramMaxOrder];
+  for (int k = 0; k < p.lm_hist_n; ++k) ids[k] = p.ngram.bos;
+  lm_row[c] = lm_dev_term(p, ids, p.label_word[c]);
+}
+
+CTC_FN void lm_dev_node(const BeamParams &p, int *hist, float *lm_arena, float *lm_row, int nid, int par, int ch,
+                        int par_state, int arc, int dst) {
+  const int H = p.lm_hist_n;
+  int ids[kNgramMaxOrder];
+  const int *hp = hist + (size_t)par * H;
+  const bool shift = p.lm_char || ch == p.space_id;
+  for (int k = 0; k < H; ++k) ids[k] = shift ? (k + 1 < H ? hp[k + 1] : 0) : hp[k];
+  if (shift) ids[H - 1] = p.lm_char ? p.label_word[ch] : p.word_of_state[par_state];
+  for (int k = 0; k < H; ++k) hist[(size_t)nid * H + k] = ids[k];
+  if (p.lm_char) {
+    for (int c = 0; c < p.V; ++c) lm_row[(size_t)nid * p.V + c] = lm_dev_term(p, ids, p.label_word[c]);
+  } else if (arc & kDictSpace) {
+    lm_arena[nid] = lm_dev_term(p, ids, p.word_of_state[dst]);
+  }
+}
+
 #if defined(CTC_EMULATE) && defined(CTC_STATS)
 struct EmuStats { long long frames, passes, walk_iters, anchors_live, evicted, anchors_new, rv_hops, created, revived,
                   hist_adds, tie_frames, sel_all_frames, rv_frames, rows, rows_skipped, cl_entries, rewalks, fb_frames, ovf_first, heur_fail,
@@ -396,8 +429,12 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
   float *const lm_row = !(LM && p.lm_char) ? nullptr
                         : p.lm_row_ptrs ? p.lm_row_ptrs[b] : p.lm_row + (size_t)b * (size_t)p.arena_stride * (size_t)V;
   c.lm_row = lm_row;
-  int *const newlist = LM ? p.newlist + (long long)b * p.lm_nl_stride : nullptr;
-  const int *const lm_upd = LM ? p.lm_upd + (long long)b * p.lm_up_stride : nullptr;
+  int *const newlist = LM && !p.lm_dev ? p.newlist + (long long)b * p.lm_nl_stride : nullptr;
+  const int *const lm_upd = LM && !p.lm_dev ? p.lm_upd + (long long)b * p.lm_up_stride : nullptr;
+  // (a streaming state keeps its histories behind its LM terms, in the same allocation: lm_arena[arena_cap ...])
+  int *const lm_hist = !(LM && p.lm_dev) ? nullptr
+                       : p.lm_arena_ptrs ? reinterpret_cast<int *>(lm_arena + arena_cap)
+                                         : p.lm_hist + (size_t)b * (size_t)p.arena_stride * (size_t)p.lm_hist_n;
   int *const s_upd = CTC_SLOT(int, U_NEWINFO);  // staging for the host's answer (free outside R4c..R5: 10 * KP ints)
   // the host's answer: (node, term) pairs -- or, for a character-based model, (node, V terms) entries that are too many
   // for the staging area and are copied from the mapped block straight into the node rows
@@ -475,7 +512,7 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
   int *const st_slots = st + kStateHeader;
   int *const st_anchors = st_slots + kSlotArrays * K;
 
-  if (LM) {
+  if (LM && !p.lm_dev) {
     // scores the host's Scorer hook computed for the nodes created by the previous launch
     CTC_PAR {
       if (tid == 0) newlist[0] = 0;
@@ -540,6 +577,13 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
         store_node(&nodes[0], root);
         if (LM) { dstate_arena[0] = p.dict_start; lm_arena[0] = 0.0f; }
       }
+    }
+    // device n-gram scorer, before the first frame of an utterance or stream: the root's history (the "<s>" padding
+    // of Scorer::make_ngram) and, for a character-based model, its row of LM terms
+    if (LM && p.lm_dev && abs_t0 == 0) {
+      for (int k = tid; k < p.lm_hist_n; k += NT) lm_hist[k] = p.ngram.bos;
+      if (p.lm_char)
+        for (int x = tid; x < V; x += NT) lm_dev_root_term(p, lm_row, x);
     }
   }
 #if !defined(CTC_EMULATE)

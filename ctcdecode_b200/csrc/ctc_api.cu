@@ -429,6 +429,8 @@ struct StreamState {
   float *lm_arena = nullptr;
   int *dstate = nullptr;
   float *lm_row = nullptr;  // character-based model: [arena_cap][V] per-node rows of LM terms
+  // ARPA scorer: order - 1, and lm_arena holds [arena_cap] terms, then [arena_cap][order - 1] LM word ids per node
+  int lm_hist_n = 0;
   TrieMirror mirror;
 };
 
@@ -443,6 +445,42 @@ static int ensure_dict_on_device(HostScorer *sc, int device) {
     CU(cudaMemcpy(sc->d_mask, sc->dict.mask.data(), sc->dict.mask.size() * 4, cudaMemcpyHostToDevice));
     sc->device = device;
   }
+  return CTCDEC_OK;
+}
+
+// The tables of an ARPA scorer and the kernel's word-id arrays in device memory, uploaded once per device.
+static int ensure_ngram_on_device(HostScorer *sc, int device) {
+  if (sc->d_ngram && sc->ngram_device != device) {
+    cudaSetDevice(sc->ngram_device); cudaFree(sc->d_ngram); sc->d_ngram = nullptr; cudaSetDevice(device);
+  }
+  if (sc->d_ngram) return CTCDEC_OK;
+  const NgramModel &m = *sc->ngram;
+  std::vector<std::pair<const void *, size_t>> parts;
+  parts.emplace_back(m.uni_prob.data(), m.uni_prob.size() * 4);
+  parts.emplace_back(m.uni_backoff.data(), m.uni_backoff.size() * 4);
+  for (int n = 2; n <= m.order; ++n) parts.emplace_back(m.tables[n - 1].data(), m.tables[n - 1].size() * sizeof(NgramEntry));
+  parts.emplace_back(sc->word_of_state.data(), sc->word_of_state.size() * 4);
+  parts.emplace_back(sc->label_word.data(), sc->label_word.size() * 4);
+  std::vector<size_t> off;
+  size_t total = 0;
+  for (const auto &pt : parts) { off.push_back(total); total += al256(pt.second); }
+  std::vector<unsigned char> staged(total);
+  for (size_t i = 0; i < parts.size(); ++i)
+    if (parts[i].second) memcpy(staged.data() + off[i], parts[i].first, parts[i].second);
+  unsigned char *d = nullptr;
+  CU(cudaMalloc(&d, total));
+  const cudaError_t e = cudaMemcpy(d, staged.data(), total, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) { cudaFree(d); return fail(CTCDEC_E_CUDA, "n-gram tables upload: %s", cudaGetErrorString(e)); }
+  NgramView v = m.view();
+  size_t i = 0;
+  v.uni_prob = reinterpret_cast<const float *>(d + off[i++]);
+  v.uni_backoff = reinterpret_cast<const float *>(d + off[i++]);
+  for (int n = 2; n <= m.order; ++n) v.table[n - 1] = reinterpret_cast<const NgramEntry *>(d + off[i++]);
+  sc->d_word_of_state = reinterpret_cast<int *>(d + off[i++]);
+  sc->d_label_word = reinterpret_cast<int *>(d + off[i++]);
+  sc->d_view = v;
+  sc->d_ngram = d;
+  sc->ngram_device = device;
   return CTCDEC_OK;
 }
 
@@ -868,8 +906,9 @@ int ctcdec_state_create_lm(const ctcdec_config *cfg, void *scorer, int device, v
   int rc = state_create(cfg, device, true, state);
   if (rc) return rc;
   StreamState *st = static_cast<StreamState *>(*state);
+  st->lm_hist_n = sc->ngram ? sc->max_order - 1 : 0;
   // node 0 (the root): dictionary start state (0) and LM term 0, reference path_trie.cpp:11-30 / :165-174
-  if (cudaMalloc(&st->lm_arena, (size_t)st->arena_cap * 4) != cudaSuccess ||
+  if (cudaMalloc(&st->lm_arena, (size_t)st->arena_cap * (1 + st->lm_hist_n) * 4) != cudaSuccess ||
       cudaMalloc(&st->dstate, (size_t)st->arena_cap * 4) != cudaSuccess ||
       cudaMemset(st->lm_arena, 0, 4) != cudaSuccess || cudaMemset(st->dstate, 0, 4) != cudaSuccess) {
     ctcdec_state_destroy(st);
@@ -963,9 +1002,12 @@ static int grow_arenas(void *const *states, int B, const int *clen, cudaStream_t
     if (sb->sc) {
       float *nl = nullptr;
       int *nd = nullptr;
-      CU(cudaMalloc(&nl, (size_t)cap * 4));
+      CU(cudaMalloc(&nl, (size_t)cap * (1 + sb->lm_hist_n) * 4));
       CU(cudaMalloc(&nd, (size_t)cap * 4));
       CU(cudaMemcpyAsync(nl, sb->lm_arena, (size_t)used * 4, cudaMemcpyDeviceToDevice, s));
+      if (sb->lm_hist_n)  // the LM histories, behind the terms
+        CU(cudaMemcpyAsync(nl + cap, sb->lm_arena + sb->arena_cap, (size_t)used * sb->lm_hist_n * 4,
+                           cudaMemcpyDeviceToDevice, s));
       CU(cudaMemcpyAsync(nd, sb->dstate, (size_t)used * 4, cudaMemcpyDeviceToDevice, s));
       CU(cudaStreamSynchronize(s));
       CU(cudaFree(sb->lm_arena));
@@ -1049,7 +1091,18 @@ static int stream_chunk_step(const ctcdec_config &cfg, Plan &pl, void *const *st
   bp.fresh = 0;
   bp.out_tokens = io.tokens; bp.out_timesteps = io.timesteps; bp.out_scores = io.scores; bp.out_lens = io.lens;
   bp.n_results = io.n_results; bp.out_T = io.out_T; bp.flags = io.flags;
-  if (sc && T > 0) {
+  if (sc && sc->ngram && T > 0) {
+    // ARPA scorer: the beam kernel computes the LM terms itself, one launch per chunk and no handshake
+    if ((rc = ensure_ngram_on_device(sc, static_cast<StreamState *>(states[0])->device))) return rc;
+    bp.dict_next = sc->d_next; bp.dict_mask = sc->d_mask; bp.dict_wc = sc->dict.wc; bp.dict_start = sc->dict.start;
+    bp.space_id = sc->space_id; bp.beta = sc->beta;
+    bp.lm_arena_ptrs = (float *const *)(io.tab + L.lmar);
+    bp.dstate_ptrs = (int *const *)(io.tab + L.dst);
+    if (sc->is_character_based) { bp.lm_char = 1; bp.lm_row_ptrs = (float *const *)(io.tab + L.rows); }
+    bp.lm_dev = 1; bp.lm_alpha = sc->alpha; bp.ngram = sc->d_view;
+    bp.word_of_state = sc->d_word_of_state; bp.label_word = sc->d_label_word; bp.lm_hist_n = sc->max_order - 1;
+    if ((rc = launch_beam(bp, pl, B, s))) return rc;
+  } else if (sc && T > 0) {
     // scorer path: one persistent launch per chunk, hand shake after EVERY frame (the frame after the chunk's last
     // one, in the next call, needs the LM terms of the nodes created now)
     int nls = 0, ups = 0;
@@ -1319,10 +1372,51 @@ int ctcdec_scorer_create(const ctcdec_scorer_hooks *hooks, double alpha, double 
   return CTCDEC_OK;
 }
 
+int ctcdec_scorer_create_arpa(const char *path, double alpha, double beta, const char *const *labels, int n_labels,
+                              void **scorer) {
+  if (!path || !labels || n_labels < 1 || !scorer) return fail(CTCDEC_E_INVALID, "bad path / labels / scorer argument");
+  if (FILE *probe = fopen(path, "rb")) fclose(probe);
+  else return fail(CTCDEC_E_INVALID, "cannot open the language model %s", path);
+  std::shared_ptr<NgramModel> m = std::make_shared<NgramModel>();
+  for (int i = 0; i < n_labels; ++i) {
+    m->labels.emplace_back(labels[i] ? labels[i] : "");
+    if (m->labels.back() == " ") m->space_id = i;  // reference Scorer::set_char_map (scorer.cpp:148-161)
+  }
+  const std::string why = load_arpa(path, *m);
+  if (!why.empty()) return fail(CTCDEC_E_UNSUPPORTED, "language model %s refused: %s", path, why.c_str());
+  std::vector<const char *> words;
+  for (const std::string &w : m->vocabulary) words.push_back(w.c_str());
+  const ctcdec_scorer_hooks hooks = {m.get(), ngram_hook_cond, ngram_hook_sent};
+  const int rc = ctcdec_scorer_create(&hooks, alpha, beta, labels, n_labels, words.data(), (int)words.size(), m->order,
+                                      m->is_character_based, scorer);
+  if (rc != CTCDEC_OK) return rc;
+  HostScorer *sc = static_cast<HostScorer *>(*scorer);
+  sc->ngram = m;
+  lm_dev_word_ids(*sc);
+  return CTCDEC_OK;
+}
+
+static int scorer_hook_call(const void *scorer, const int32_t *labels, int n, double *out, bool sent) {
+  if (!scorer || (!labels && n > 0) || n < 0 || !out) return fail(CTCDEC_E_INVALID, "bad scorer / labels / out argument");
+  const HostScorer *sc = static_cast<const HostScorer *>(scorer);
+  for (int i = 0; i < n; ++i)
+    if (labels[i] < 0 || labels[i] >= (int)sc->labels.size())
+      return fail(CTCDEC_E_INVALID, "label %d at position %d is outside [0, %d)", labels[i], i, (int)sc->labels.size());
+  *out = (sent ? sc->hooks.sent_log_prob : sc->hooks.cond_log_prob)(sc->hooks.ctx, labels, n);
+  return CTCDEC_OK;
+}
+int ctcdec_scorer_cond_log_prob(const void *scorer, const int32_t *labels, int n, double *out) {
+  return scorer_hook_call(scorer, labels, n, out, false);
+}
+int ctcdec_scorer_sent_log_prob(const void *scorer, const int32_t *labels, int n, double *out) {
+  return scorer_hook_call(scorer, labels, n, out, true);
+}
+
 int ctcdec_scorer_destroy(void *scorer) {
   if (!scorer) return CTCDEC_OK;
   HostScorer *sc = static_cast<HostScorer *>(scorer);
   if (sc->d_next) { cudaSetDevice(sc->device); cudaFree(sc->d_next); cudaFree(sc->d_mask); }
+  if (sc->d_ngram) { cudaSetDevice(sc->ngram_device); cudaFree(sc->d_ngram); }
   delete sc;
   return CTCDEC_OK;
 }
@@ -1334,6 +1428,16 @@ int ctcdec_scorer_reset_params(void *scorer, double alpha, double beta) {
   HostScorer *sc = static_cast<HostScorer *>(scorer);
   sc->alpha = (double)(float)alpha;  // reference Scorer::reset_params(float, float) (scorer.cpp:122-125): both values
   sc->beta = (double)(float)beta;    // pass through float32 (the constructor takes doubles)
+  return CTCDEC_OK;
+}
+
+// ARPA scorer: the device keeps the last order - 1 LM word ids of every trie node, batch x (1 + beam x frames) x
+// (order - 1) ints
+static int lm_hist_bytes(const HostScorer *sc, const Plan &pl, int B, size_t *bytes) {
+  *bytes = sc->ngram ? (size_t)B * pl.arena_stride * (size_t)(sc->max_order - 1) * 4 : 0;
+  if (*bytes > ((size_t)64 << 30))
+    return fail(CTCDEC_E_UNSUPPORTED, "n-gram scorer: %zu bytes of per-node LM histories (batch x (1 + beam x frames) x "
+                "(order - 1) x 4)", *bytes);
   return CTCDEC_OK;
 }
 
@@ -1354,6 +1458,7 @@ struct LmBuffers {
   float *lm_arena;               // [B][arena_stride] LM term of each trie node
   int *dstate;                   // [B][arena_stride] dictionary state of each trie node
   float *lm_row;                 // character-based model: [B][arena_stride][V] rows of LM terms, else NULL
+  int *lm_hist;                  // ARPA scorer: [B][arena_stride][order - 1] LM word ids of each trie node, else NULL
   int32_t *tokens, *timesteps;   // [B, K, T]
   float *scores;                 // [B, K] (the raw prefix scores: the caller rescores them with lm_rescore_batch)
   int32_t *lens, *n_results, *flags;
@@ -1363,27 +1468,15 @@ struct LmBuffers {
 // entry points, which stage around it (ctcdec_decode_batch_lm_host) or not (ctcdec_decode_batch_lm_device).  Uploads
 // the dictionary, prepares the pinned exchange blocks of `c`, runs the prune scan, the beam kernel (persistent with
 // the per-frame host handshake, or one launch per frame with CTCDEC_LM_PER_FRAME) and enqueues the finalize kernel.
-// seq_lens: the host array (the handshake serves need[b] frames of utterance b).  The caller holds g_mu[device].
+// An ARPA scorer (ctcdec_scorer_create_arpa) skips the exchange: its tables go to the device and the one beam launch
+// computes the LM terms itself.  seq_lens: the host array (the handshake serves need[b] frames of utterance b).  The
+// caller holds g_mu[device].
 static int lm_batch_step(const ctcdec_config *cfg, const Plan &pl, HostScorer *sc, DevCache &c, int device,
                          const int32_t *seq_lens, int B, int T, const LmBuffers &io, cudaStream_t s) {
   const int V = cfg->vocab_size, K = cfg->beam_size;
   int rc = ensure_dict_on_device(sc, device);
-  if (rc) return rc;
-  int nls = 0, ups = 0;
-  exchange_strides(K, exchange_row_len(*sc), &nls, &ups);
+  if (rc || (sc->ngram && (rc = ensure_ngram_on_device(sc, device)))) return rc;
   const bool lm_char = sc->is_character_based != 0;
-  if ((rc = ensure_pinned(c, 0, (size_t)B * nls * 4))) return rc;
-  if ((rc = ensure_pinned(c, 1, (size_t)B * ups * 4))) return rc;
-  if ((rc = ensure_pinned(c, 2, 256))) return rc;
-  int *h_newlist = (int *)c.pin[0], *h_upd = (int *)c.pin[1], *hs_abort = (int *)c.pin[2];
-  for (int b = 0; b < B; ++b) { memset(h_newlist + (size_t)b * nls, 0, 16); memset(h_upd + (size_t)b * ups, 0, 8); }
-  if (lm_char) {  // the root's row of LM terms: the first entry every CTA picks up before frame 0
-    std::vector<int> scratch;
-    lm_char_root_entry(*sc, sc->cond_caches[0], h_upd, scratch);
-    for (int b = 1; b < B; ++b) memcpy(h_upd + (size_t)b * ups, h_upd, (size_t)(3 + V) * 4);
-  }
-  *hs_abort = 0;
-
   CU(cudaMemsetAsync(io.flags, 0, (size_t)B * 4, s));
   float *lp = reinterpret_cast<float *>(io.ws + pl.off_lp);
   uint16_t *idx = pl.sorted ? reinterpret_cast<uint16_t *>(io.ws + pl.off_idx) : nullptr;
@@ -1403,6 +1496,29 @@ static int lm_batch_step(const ctcdec_config *cfg, const Plan &pl, HostScorer *s
   bp.space_id = sc->space_id; bp.beta = sc->beta; bp.lm_arena = io.lm_arena; bp.dstate_arena = io.dstate;
   bp.lm_char = lm_char ? 1 : 0; bp.lm_row = lm_char ? io.lm_row : nullptr;
   bp.timing = g_prof.timing;
+  if (sc->ngram) {
+    // ARPA scorer: the beam kernel computes the LM terms itself, so ONE launch decodes the batch, with no exchange
+    // blocks, host workers or handshake
+    bp.lm_dev = 1; bp.lm_alpha = sc->alpha; bp.ngram = sc->d_view;
+    bp.word_of_state = sc->d_word_of_state; bp.label_word = sc->d_label_word;
+    bp.lm_hist_n = sc->max_order - 1; bp.lm_hist = io.lm_hist;
+    bp.t0 = 0; bp.nframes = 0; bp.fresh = 1;
+    if ((rc = launch_beam(bp, pl, B, s))) return rc;
+    return launch_finalize(bp, B, s);
+  }
+  int nls = 0, ups = 0;
+  exchange_strides(K, exchange_row_len(*sc), &nls, &ups);
+  if ((rc = ensure_pinned(c, 0, (size_t)B * nls * 4))) return rc;
+  if ((rc = ensure_pinned(c, 1, (size_t)B * ups * 4))) return rc;
+  if ((rc = ensure_pinned(c, 2, 256))) return rc;
+  int *h_newlist = (int *)c.pin[0], *h_upd = (int *)c.pin[1], *hs_abort = (int *)c.pin[2];
+  for (int b = 0; b < B; ++b) { memset(h_newlist + (size_t)b * nls, 0, 16); memset(h_upd + (size_t)b * ups, 0, 8); }
+  if (lm_char) {  // the root's row of LM terms: the first entry every CTA picks up before frame 0
+    std::vector<int> scratch;
+    lm_char_root_entry(*sc, sc->cond_caches[0], h_upd, scratch);
+    for (int b = 1; b < B; ++b) memcpy(h_upd + (size_t)b * ups, h_upd, (size_t)(3 + V) * 4);
+  }
+  *hs_abort = 0;
   // The per-frame exchange with the host goes through pinned, device-mapped host memory (unified addressing):
   // the kernel reads the few LM updates and writes the new-node list straight over PCIe, so a frame costs one
   // launch and one stream synchronisation, no memcpy calls.
@@ -1497,6 +1613,8 @@ int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const fl
   const size_t lm_bytes = al256((size_t)B * pl.arena_stride * 4) * 2;
   size_t row_bytes = 0;
   if ((rc = lm_row_bytes(sc, pl, B, &row_bytes))) return rc;
+  size_t hist_bytes = 0;
+  if ((rc = lm_hist_bytes(sc, pl, B, &hist_bytes))) return rc;
   if ((rc = ensure(c, 0, n_probs * 4 + 256))) return rc;
   if ((rc = ensure(c, 1, (size_t)B * 4 + 256))) return rc;
   if ((rc = ensure(c, 2, n_out * 4 + 256))) return rc;
@@ -1505,6 +1623,7 @@ int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const fl
   if ((rc = ensure(c, 5, pl.total + 512))) return rc;
   if ((rc = ensure(c, 7, lm_bytes + 512))) return rc;
   if (row_bytes && (rc = ensure(c, 8, row_bytes + 256))) return rc;
+  if (hist_bytes && (rc = ensure(c, 9, hist_bytes + 256))) return rc;
   float *d_probs = (float *)c.buf[0];
   int *d_lens_in = seq_lens ? (int *)c.buf[1] : nullptr;
   int *d_tok = (int *)c.buf[2], *d_ts = (int *)c.buf[3];
@@ -1522,6 +1641,7 @@ int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const fl
   io.lm_arena = (float *)lmb;
   io.dstate = (int *)(lmb + al256((size_t)B * pl.arena_stride * 4));
   io.lm_row = row_bytes ? (float *)c.buf[8] : nullptr;
+  io.lm_hist = hist_bytes ? (int *)c.buf[9] : nullptr;
   io.tokens = d_tok; io.timesteps = d_ts; io.scores = d_scores; io.lens = d_lens; io.n_results = d_nres;
   io.flags = d_flags;
   if ((rc = lm_batch_step(cfg, pl, sc, c, device, seq_lens, B, T, io, s))) return rc;
@@ -1572,17 +1692,19 @@ int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const fl
 }
 
 // Device scratch of ctcdec_decode_batch_lm_device: the plan's regions, then the per-node LM terms and dictionary
-// states, for a character-based model the per-node rows of LM terms, and the device copy of seq_lens.
-struct LmWorkspace { size_t lm_arena, dstate, rows, lens, total; };
+// states, for a character-based model the per-node rows of LM terms, for an ARPA scorer the per-node LM histories, and
+// the device copy of seq_lens.
+struct LmWorkspace { size_t lm_arena, dstate, rows, hist, lens, total; };
 static int lm_workspace(const HostScorer *sc, const Plan &pl, int B, LmWorkspace *w) {
-  size_t row_bytes = 0;
-  const int rc = lm_row_bytes(sc, pl, B, &row_bytes);
-  if (rc) return rc;
+  size_t row_bytes = 0, hist_bytes = 0;
+  int rc = lm_row_bytes(sc, pl, B, &row_bytes);
+  if (rc || (rc = lm_hist_bytes(sc, pl, B, &hist_bytes))) return rc;
   const size_t node_bytes = al256((size_t)B * pl.arena_stride * 4);
   w->lm_arena = pl.total;
   w->dstate = w->lm_arena + node_bytes;
   w->rows = w->dstate + node_bytes;
-  w->lens = w->rows + al256(row_bytes);
+  w->hist = w->rows + al256(row_bytes);
+  w->lens = w->hist + al256(hist_bytes);
   w->total = w->lens + al256((size_t)B * 4);
   return CTCDEC_OK;
 }
@@ -1654,6 +1776,7 @@ int ctcdec_decode_batch_lm_device(const ctcdec_config *cfg, void *scorer, const 
   io.lm_arena = reinterpret_cast<float *>(ws + w.lm_arena);
   io.dstate = reinterpret_cast<int *>(ws + w.dstate);
   io.lm_row = sc->is_character_based ? reinterpret_cast<float *>(ws + w.rows) : nullptr;
+  io.lm_hist = sc->ngram ? reinterpret_cast<int *>(ws + w.hist) : nullptr;
   io.tokens = tokens; io.timesteps = timesteps; io.scores = scores; io.lens = lens; io.n_results = n_results;
   io.flags = flags;
   if ((rc = lm_batch_step(cfg, pl, sc, c, device, seq_lens, B, T, io, s))) return rc;

@@ -18,12 +18,14 @@
 #pragma once
 #include <cstdint>
 #include <cstring>
+#include <memory>
 #include <string>
 #include <thread>
 #include <unordered_map>
 #include <vector>
 
 #include "../../include/ctcdecode_b200.h"
+#include "ngram_arpa.h"
 
 namespace ctc {
 
@@ -137,11 +139,51 @@ struct HostScorer {
   int max_order, is_character_based, space_id;
   std::vector<std::string> labels;
   Dictionary dict;
+  // the model behind the hooks of a scorer built from an ARPA file (ctcdec_scorer_create_arpa; hooks.ctx points to
+  // it), null for a scorer whose hooks the caller supplies
+  std::shared_ptr<const NgramModel> ngram;
+  // what the beam kernel needs besides the tables to compute an ARPA scorer's terms itself (BeamParams::lm_dev):
+  // word-based, the word id each dictionary state completes with a space (0 if none); character-based, each label's
+  std::vector<int> word_of_state, label_word;
+  // device copies of the tables and of those two arrays (one allocation, ensure_ngram_on_device)
+  void *d_ngram = nullptr;
+  int ngram_device = -1;
+  NgramView d_view;
+  int *d_word_of_state = nullptr, *d_label_word = nullptr;
   // device copies of the dictionary (CUDA library only)
   int *d_next = nullptr;
   uint32_t *d_mask = nullptr;
   int device = -1;
 };
+
+// An ARPA scorer's word ids for the beam kernel (BeamParams::lm_dev): word-based, the word each dictionary state completes
+// with a space (the dictionary is a trie from its start state: spell every state); character-based, each label's.
+static inline void lm_dev_word_ids(HostScorer &sc) {
+  const NgramModel &m = *sc.ngram;
+  const Dictionary &d = sc.dict;
+  if (sc.is_character_based) {
+    sc.label_word.clear();
+    for (const std::string &l : sc.labels) sc.label_word.push_back(m.id_of(l));
+    return;
+  }
+  sc.word_of_state.assign(d.states(), 0);
+  std::vector<std::string> spelled(d.states());
+  std::vector<int> todo(1, d.start);
+  while (!todo.empty()) {
+    const int st = todo.back();
+    todo.pop_back();
+    for (int c = 0; c < d.V; ++c) {
+      const int nx = d.next[(size_t)st * d.V + c];
+      if (nx < 0) continue;
+      if (c == sc.space_id) {
+        if (d.fin[nx]) sc.word_of_state[st] = m.id_of(spelled[st]);
+        continue;
+      }
+      spelled[nx] = spelled[st] + sc.labels[c];
+      todo.push_back(nx);
+    }
+  }
+}
 
 // Per-utterance host mirror of the trie: enough to spell the prefix of any node.
 struct TrieMirror {

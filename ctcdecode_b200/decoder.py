@@ -15,7 +15,8 @@ Differences from the reference, all additive:
     of the last call (the reference has no equivalent; see include/ctcdecode_b200.h).
   * ``model_path`` (word-based KenLM models): the language model stays on the host behind a hook; the real Scorer
     comes from a provider library (``scorer_provider=`` / CTCDECODE_B200_SCORER_PROVIDER, see scorer.py and
-    INTEGRATION.md; providers/ builds one from the reference's own Scorer + KenLM).  CUDA probabilities and logits
+    INTEGRATION.md; providers/ builds one from the reference's own Scorer + KenLM).  ``scorer_provider="device"``
+    needs no provider: the library reads an ARPA file itself and reproduces the reference Scorer bit for bit.  CUDA probabilities and logits
     stay on the GPU with a scorer too (ctcdec_decode_batch_lm_device); that call returns when the results are in place,
     because the host answers the beam kernel's per-frame LM handshake while it runs.  The online decoder takes a
     scorer too (device-resident states, one persistent launch per chunk).  Character-based models are detected like
@@ -81,8 +82,8 @@ class _Base(object):
         self.last_n_results = None
         _native.load()
         if model_path:
-            from .scorer import ProviderScorer
-            self._scorer = ProviderScorer(self._labels, model_path, alpha, beta, scorer_provider)
+            from .scorer import make_scorer
+            self._scorer = make_scorer(self._labels, model_path, alpha, beta, scorer_provider)
 
     def _device_index(self, probs=None):
         if probs is not None and probs.is_cuda:

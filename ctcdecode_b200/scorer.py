@@ -16,6 +16,10 @@ small stub of INTEGRATION.md section 6 -- that owns the real ``Scorer`` (KenLM) 
 providers/ in this repository holds exactly that stub (kenlm_provider.cpp) and the recipe (Makefile) that builds it
 from the reference's sources where they lie: providers/_build/libkenlm_provider.so, used when present.  Another
 provider is chosen with ``scorer_provider=`` or the environment variable CTCDECODE_B200_SCORER_PROVIDER.
+
+``scorer_provider="device"`` (or CTCDECODE_B200_SCORER_PROVIDER=device) needs no provider: ``ArpaScorer`` has the
+library read an ARPA text file itself (ctcdec_scorer_create_arpa).  Its hooks reproduce the reference Scorer over
+KenLM bit for bit; a model they cannot reproduce exactly (a KenLM binary file, order above 6, ...) is refused.
 """
 import ctypes
 import os
@@ -24,6 +28,57 @@ from . import _native
 
 DEFAULT_PROVIDER = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "providers", "_build",
                                 "libkenlm_provider.so")
+
+
+DEVICE = "device"
+
+
+def make_scorer(labels, model_path, alpha, beta, provider=None):
+    """The scorer for ``model_path``: the library's own ARPA scorer for provider "device", else a provider's."""
+    provider = provider or os.environ.get("CTCDECODE_B200_SCORER_PROVIDER")
+    if provider == DEVICE:
+        return ArpaScorer(labels, model_path, alpha, beta)
+    return ProviderScorer(labels, model_path, alpha, beta, provider)
+
+
+class ArpaScorer(object):
+    """The library-side scorer built from an ARPA file by the library itself (no provider library, no KenLM)."""
+
+    def __init__(self, labels, model_path, alpha, beta):
+        self.handle = None
+        if not os.path.exists(model_path):
+            raise FileNotFoundError(model_path)
+        self._lib = _native.load()
+        labels = list(labels)
+        lab = (ctypes.c_char_p * len(labels))(*[s.encode() for s in labels])
+        path = model_path.encode() if isinstance(model_path, str) else model_path
+        handle = ctypes.c_void_p()
+        _native.check(self._lib.ctcdec_scorer_create_arpa(path, float(alpha), float(beta), lab, len(labels),
+                                                          ctypes.byref(handle)))
+        self.handle = handle.value
+
+    def is_character_based(self):
+        return int(self._lib.ctcdec_scorer_is_character_based(self.handle))
+
+    def max_order(self):
+        return int(self._lib.ctcdec_scorer_max_order(self.handle))
+
+    def dict_size(self):
+        return int(self._lib.ctcdec_scorer_dict_size(self.handle))
+
+    def reset_params(self, alpha, beta):
+        _native.check(self._lib.ctcdec_scorer_reset_params(self.handle, float(alpha), float(beta)))
+
+    def release(self):
+        if getattr(self, "handle", None):
+            self._lib.ctcdec_scorer_destroy(self.handle)
+            self.handle = None
+
+    def __del__(self):
+        try:
+            self.release()
+        except Exception:
+            pass
 
 
 class ProviderScorer(object):

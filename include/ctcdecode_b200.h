@@ -170,6 +170,27 @@ typedef struct ctcdec_scorer_hooks {
 int ctcdec_scorer_create(const ctcdec_scorer_hooks *hooks, double alpha, double beta, const char *const *labels,
                          int n_labels, const char *const *words, int n_words, int max_order, int is_character_based,
                          void **scorer);
+/* The same scorer from an ARPA text file, with no hook to supply: the library reads the n-gram tables itself and its
+ * own hooks reproduce the reference Scorer over KenLM (Scorer::get_log_cond_prob / get_sent_log_prob, scorer.cpp:74-120)
+ * bit for bit: the longest matching n-gram, KenLM's float sum of context backoffs in KenLM's order, "<s>" padding scored
+ * as words, any out-of-vocabulary word -1000.  Word-based or character-based is read from the vocabulary as
+ * scorer.cpp:61-71 does; max_order is the file's order; the dictionary is built from the unigrams.  Every entry point
+ * that takes a scorer takes this one, and the accessors below behave as for a hook scorer.  The n-gram tables go to the
+ * device once per device, and the beam kernel computes the LM terms of the trie nodes it creates itself: the offline
+ * entries and ctcdec_decode_stream_host run without the per-frame host handshake (one launch per batch or chunk), and
+ * the device keeps the last max_order - 1 word ids of every node, batch x (1 + beam x frames) x (max_order - 1) x 4
+ * bytes (CTCDEC_E_UNSUPPORTED beyond 64 GiB).  The read-out rescoring stays on the host, through this scorer's hooks.
+ * Refused with CTCDEC_E_UNSUPPORTED, the reason in ctcdec_last_error(), anything the tables cannot reproduce exactly:
+ * a KenLM binary file or other non-ARPA input, order 1 or above 6, counts that disagree with the sections, a malformed
+ * line, a duplicate entry, an n-gram word missing from the unigrams, no <s> or </s>, an n-gram whose context or suffix
+ * n-gram is missing (KenLM would fill it in on load), a positive log-prob, a NaN or +inf log-prob, a non-finite
+ * backoff.  A file that cannot be opened is CTCDEC_E_INVALID. */
+int ctcdec_scorer_create_arpa(const char *path, double alpha, double beta, const char *const *labels, int n_labels,
+                              void **scorer);
+/* Diagnostic: the scorer's hooks on one label-id prefix -- cond_log_prob and sent_log_prob of ctcdec_scorer_hooks, for a
+ * hook scorer or an ARPA scorer.  Labels must lie in [0, n_labels). */
+int ctcdec_scorer_cond_log_prob(const void *scorer, const int32_t *labels, int n, double *out);
+int ctcdec_scorer_sent_log_prob(const void *scorer, const int32_t *labels, int n, double *out);
 /* Replaces: paddle_release_scorer, is_character_based, get_max_order, get_dict_size, reset_params
  * (binding.cpp:267-287). */
 int ctcdec_scorer_destroy(void *scorer);
@@ -191,7 +212,9 @@ int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const fl
 /* Bytes of device scratch ctcdec_decode_batch_lm_device needs for a [B, T, V] batch with this scorer: the regions of
  * ctcdec_workspace_bytes' plan, then the LM term and the dictionary state of every trie node (2 x batch x (1 + beam x
  * T) x 4 bytes, each 256-byte aligned), for a character-based model the per-node rows of LM terms (batch x (1 + beam x
- * T) x V x 4, CTCDEC_E_UNSUPPORTED beyond 64 GiB), and a device copy of seq_lens.  Checks the scorer and the shape
+ * T) x V x 4, CTCDEC_E_UNSUPPORTED beyond 64 GiB), for a scorer from ctcdec_scorer_create_arpa the per-node LM
+ * histories (batch x (1 + beam x T) x (max_order - 1) x 4, CTCDEC_E_UNSUPPORTED beyond 64 GiB), and a device copy of
+ * seq_lens.  Checks the scorer and the shape
  * like the decode does: the same refusals, no device needed. */
 int ctcdec_lm_workspace_bytes(const ctcdec_config *cfg, const void *scorer, int B, int T, size_t *bytes);
 

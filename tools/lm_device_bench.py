@@ -6,7 +6,14 @@ beta 1.0) through CTCBeamDecoder three ways:
   device          CUDA probabilities through the device entry point (ctcdec_decode_batch_lm_device)
   logits_f16      decode_logits of fp16 logits (the device entry, the log-softmax taken by the scan kernel)
 
-    python tools/lm_device_bench.py [--reps N] [--device I]
+    python tools/lm_device_bench.py [--reps N] [--device I] [--scorer hook|device]
+
+--scorer device times the library's own ARPA scorer (scorer_provider="device": the beam kernel computes the LM terms,
+no per-frame host handshake) against the hook scorer on the same CUDA probabilities instead:
+
+  hook            the reference's Scorer behind the hook, CUDA probabilities (ctcdec_decode_batch_lm_device)
+  ngram           the device scorer, CUDA probabilities (the same entry point)
+  ngram_host      the device scorer, CPU probabilities (ctcdec_decode_batch_lm_host)
 
 Every path is warmed up, then timed N times in alternating rounds with a host clock around the call (each call
 returns synchronised, with CPU results).  Prints one JSON line: per path the median and the spread of the call time
@@ -51,6 +58,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5, help="timed calls per path")
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--scorer", choices=["hook", "device"], default="hook",
+                    help="hook: the three input paths of the hook scorer; device: the device scorer against the hook")
     args = ap.parse_args()
     dev = torch.device("cuda", args.device)
     torch.cuda.set_device(dev)
@@ -61,15 +70,23 @@ def main():
     logits = probs_d.clamp_min(1e-20).log().mul(1.25).half()
     dec = CTCBeamDecoder(L29, model_path=TINY_LM, alpha=cfg["alpha"], beta=cfg["beta"], beam_width=cfg["beam"],
                          cutoff_top_n=cfg["cutoff_top_n"], cutoff_prob=cfg["cutoff_prob"], scorer_provider=PROVIDER)
-    paths = {"host": lambda: dec.decode(probs), "device": lambda: dec.decode(probs_d),
-             "logits_f16": lambda: dec.decode_logits(logits)}
+    paths = {"host": (dec, lambda: dec.decode(probs)), "device": (dec, lambda: dec.decode(probs_d)),
+             "logits_f16": (dec, lambda: dec.decode_logits(logits))}
+    compared = ("host", "device")
+    if args.scorer == "device":
+        ndec = CTCBeamDecoder(L29, model_path=TINY_LM, alpha=cfg["alpha"], beta=cfg["beta"], beam_width=cfg["beam"],
+                              cutoff_top_n=cfg["cutoff_top_n"], cutoff_prob=cfg["cutoff_prob"], scorer_provider="device")
+        paths = {"hook": (dec, lambda: dec.decode(probs_d)), "ngram": (ndec, lambda: ndec.decode(probs_d)),
+                 "ngram_host": (ndec, lambda: ndec.decode(probs))}
+        compared = ("hook", "ngram")
 
     def call(name):
+        d, fn = paths[name]
         t0 = time.perf_counter()
-        res = paths[name]()
+        res = fn()
         torch.cuda.synchronize(dev)
         dt = time.perf_counter() - t0
-        return dt, list(res) + [dec.last_n_results.clone(), dec.last_flags.clone()]
+        return dt, list(res) + [d.last_n_results.clone(), d.last_flags.clone()]
 
     outs, times = {}, {name: [] for name in paths}
     for name in paths:
@@ -81,12 +98,14 @@ def main():
             times[name].append(dt)
     legs = {name: {"ms_median": 1e3 * statistics.median(t), "ms_min": 1e3 * min(t), "ms_max": 1e3 * max(t),
                    "utterances_per_s": B / statistics.median(t), "calls": len(t)} for name, t in times.items()}
-    same = identical(outs["host"], outs["device"])
-    print(json.dumps({"workload": cfg["name"], "card": card_info(args.device), "paths": legs,
-                      "host_device_identical": bool(same),
+    same = identical(outs[compared[0]], outs[compared[1]])
+    if args.scorer == "device":
+        same = same and identical(outs["ngram"], outs["ngram_host"])
+    print(json.dumps({"workload": cfg["name"], "scorer": args.scorer, "card": card_info(args.device), "paths": legs,
+                      "%s_%s_identical" % compared: bool(same),
                       "note": "host clock around each call, which returns synchronised with CPU results; paths "
                               "alternate within each round"}), flush=True)
-    assert same, "host and device entry points gave different results"
+    assert same, "%s and %s gave different results" % compared
 
 
 if __name__ == "__main__":
