@@ -61,7 +61,12 @@ _SIGNATURES = {
     "ctcdec_decode_batch_lm_device": (ctypes.c_int, [ctypes.POINTER(Config), _vp, _vp, ctypes.c_int, _vp, ctypes.c_int,
                                                      ctypes.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
                                                      ctypes.c_size_t, _vp]),
-    "ctcdec_state_create": (ctypes.c_int, [ctypes.POINTER(Config), ctypes.c_int, ctypes.POINTER(_vp)]),
+    "ctcdec_decode_batch_lm_device_async": (ctypes.c_int, [ctypes.POINTER(Config), _vp, _vp, ctypes.c_int, _vp,
+                                                           ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, _vp,
+                                                           _vp, _vp, ctypes.c_size_t, _vp]),
+    "ctcdec_scorer_rescore_rows": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
+                                                  ctypes.c_int]),
+    "ctcdec_state_create":(ctypes.c_int, [ctypes.POINTER(Config), ctypes.c_int, ctypes.POINTER(_vp)]),
     "ctcdec_state_create_lm": (ctypes.c_int, [ctypes.POINTER(Config), _vp, ctypes.c_int, ctypes.POINTER(_vp)]),
     "ctcdec_state_destroy": (ctypes.c_int, [_vp]),
     "ctcdec_state_frames": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int)]),

@@ -99,6 +99,21 @@ __global__ void stream_table_kernel(const StreamTabArgs a) {
   reinterpret_cast<int *>(a.tab + a.L.lens)[b] = a.len[i];
 }
 
+// Read-out of an ARPA scorer's results (ngram_readout_row, reference DecoderState::decode): one thread per [B, K] result
+// row, rows p >= n_results[b] skipped, scores rescored in place.  Each row is a serial chain of hash probes (about
+// words x order of them).
+constexpr int kReadoutThreads = 128;
+__global__ void __launch_bounds__(kReadoutThreads) lm_readout_kernel(const NgramView m, const NgramFront f, double alpha,
+                                                                     double beta, const int32_t *tokens,
+                                                                     const int32_t *lens, const int32_t *n_results,
+                                                                     float *scores, int B, int K, int row_stride) {
+  const long long r = (long long)blockIdx.x * kReadoutThreads + threadIdx.x;
+  if (r >= (long long)B * K) return;
+  const int b = (int)(r / K), p = (int)(r % K);
+  if (p >= n_results[b]) return;
+  scores[r] = ngram_readout_row(m, f, tokens + r * row_stride, lens[r], scores[r], alpha, beta);
+}
+
 __global__ void selftest_math_f64_kernel(int which, const double *x, const double *x2, double *y, size_t n) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
     y[i] = which == 0 ? exp_glibc_nonpos(x[i]) : which == 1 ? log_glibc(x[i]) : lse_d(x[i], x2[i]);
@@ -141,6 +156,11 @@ static int fail(int code, const char *fmt, ...) {
 // utterances the calling thread is about to have in flight together (host entry point: all its groups)
 static thread_local int g_batch_in_flight = 0;
 
+// set while ctcdec_decode_batch_lm_device_async enqueues into a stream that is being captured: a kernel whose dynamic
+// shared-memory limit has not been raised on this device yet is refused instead of raised
+static thread_local bool g_capturing = false;
+static const char kCaptureFirst[] = "decode once outside the capture first";
+
 // the kernels raise CTCDEC_FLAG_ERR_ARENA for an utterance whose node arena / anchor table ran out or whose scorer
 // handshake was abandoned: its results are not valid, so the host entry points fail instead of returning them
 static int check_error_flags(const int *flags, int B) {
@@ -171,6 +191,7 @@ static int launch_beam_k(const BeamParams &bp, int B, cudaStream_t s) {
   CU(cudaGetDevice(&dev));
   const int smem_bytes = bp.L.total + (TIMING ? 4096 : 0);  // TIMING: [16][32] per-warp counters behind the layout
   if (smem_bytes > limit[dev & 63].load(std::memory_order_acquire)) {
+    if (g_capturing) return fail(CTCDEC_E_UNSUPPORTED, "beam kernel not prepared on device %d: %s", dev, kCaptureFirst);
     std::lock_guard<std::mutex> lk(limit_mu);  // (check again under the lock: two host threads, same device)
     if (smem_bytes > limit[dev & 63].load(std::memory_order_acquire)) {
       CU(cudaFuncSetAttribute(beam_kernel<NT, SORTED, LM, KPT, TIMING>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
@@ -252,6 +273,7 @@ static int launch_prune_k(const PruneParams &pp, int grid, int threads, size_t s
     int dev = 0;
     CU(cudaGetDevice(&dev));
     if ((int)smem > limit[dev & 63].load(std::memory_order_acquire)) {
+      if (g_capturing) return fail(CTCDEC_E_UNSUPPORTED, "prune kernel not prepared on device %d: %s", dev, kCaptureFirst);
       std::lock_guard<std::mutex> lk(limit_mu);
       if ((int)smem > limit[dev & 63].load(std::memory_order_acquire)) {
         CU(cudaFuncSetAttribute(prune_kernel<SORTED, KPL, LOGITS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -308,8 +330,20 @@ static int launch_prune(const ctcdec_config *cfg, const Plan &pl, const PruneInp
 
 static int launch_finalize(const BeamParams &bp, int B, cudaStream_t s) {
   const size_t smem = finalize_smem_bytes(bp.K);
-  if (smem > 48 * 1024)
-    CU(cudaFuncSetAttribute(finalize_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (smem > 48 * 1024) {
+    static std::atomic<int> limit[64];
+    static std::mutex limit_mu;
+    int dev = 0;
+    CU(cudaGetDevice(&dev));
+    if ((int)smem > limit[dev & 63].load(std::memory_order_acquire)) {
+      if (g_capturing) return fail(CTCDEC_E_UNSUPPORTED, "finalize kernel not prepared on device %d: %s", dev, kCaptureFirst);
+      std::lock_guard<std::mutex> lk(limit_mu);
+      if ((int)smem > limit[dev & 63].load(std::memory_order_acquire)) {
+        CU(cudaFuncSetAttribute(finalize_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        limit[dev & 63].store((int)smem, std::memory_order_release);
+      }
+    }
+  }
   // 1024 threads: the backtrace is a latency-bound pointer chase, its only resource is chains in flight
   finalize_kernel<1024><<<B, 1024, smem, s>>>(bp);
   CU(cudaGetLastError());
@@ -461,6 +495,10 @@ static int ensure_ngram_on_device(HostScorer *sc, int device) {
   for (int n = 2; n <= m.order; ++n) parts.emplace_back(m.tables[n - 1].data(), m.tables[n - 1].size() * sizeof(NgramEntry));
   parts.emplace_back(sc->word_of_state.data(), sc->word_of_state.size() * 4);
   parts.emplace_back(sc->label_word.data(), sc->label_word.size() * 4);
+  parts.emplace_back(m.label_bytes.data(), m.label_bytes.size());
+  parts.emplace_back(m.label_off.data(), m.label_off.size() * 4);
+  parts.emplace_back(m.word_bytes.data(), m.word_bytes.size());
+  parts.emplace_back(m.words.data(), m.words.size() * sizeof(NgramWordSlot));
   std::vector<size_t> off;
   size_t total = 0;
   for (const auto &pt : parts) { off.push_back(total); total += al256(pt.second); }
@@ -478,9 +516,27 @@ static int ensure_ngram_on_device(HostScorer *sc, int device) {
   for (int n = 2; n <= m.order; ++n) v.table[n - 1] = reinterpret_cast<const NgramEntry *>(d + off[i++]);
   sc->d_word_of_state = reinterpret_cast<int *>(d + off[i++]);
   sc->d_label_word = reinterpret_cast<int *>(d + off[i++]);
+  NgramFront f = m.front();
+  f.label_bytes = d + off[i++];
+  f.label_off = reinterpret_cast<const int32_t *>(d + off[i++]);
+  f.word_bytes = d + off[i++];
+  f.words = reinterpret_cast<const NgramWordSlot *>(d + off[i++]);
   sc->d_view = v;
+  sc->d_front = f;
   sc->d_ngram = d;
   sc->ngram_device = device;
+  return CTCDEC_OK;
+}
+
+// Enqueues the read-out of an ARPA scorer's [B, K] result rows (row_stride columns each) on s; the scorer's tables must
+// be on the current device.  alpha and beta are the scorer's values now.
+static int launch_readout(const HostScorer *sc, const int32_t *tokens, const int32_t *lens, const int32_t *n_results,
+                          float *scores, int B, int K, int row_stride, cudaStream_t s) {
+  const long long rows = (long long)B * K;
+  if (rows == 0) return CTCDEC_OK;
+  lm_readout_kernel<<<(unsigned)((rows + kReadoutThreads - 1) / kReadoutThreads), kReadoutThreads, 0, s>>>(
+      sc->d_view, sc->d_front, sc->alpha, sc->beta, tokens, lens, n_results, scores, B, K, row_stride);
+  CU(cudaGetLastError());
   return CTCDEC_OK;
 }
 
@@ -1270,11 +1326,12 @@ int ctcdec_decode_stream_device(const void *probs, int dtype, const int32_t *seq
   int rc = check_states(states, B);
   if (rc) return rc;
   StreamState *s0 = static_cast<StreamState *>(states[0]);
-  if (s0->sc)
+  HostScorer *const sc = s0->sc;
+  if (sc && !sc->ngram)
     return fail(CTCDEC_E_UNSUPPORTED, "states with a scorer need the per-frame host handshake: use ctcdec_decode_stream_host");
   const ctcdec_config cfg = s0->cfg;
   Plan pl;
-  if ((rc = make_plan(&cfg, B, T, &pl))) return rc;
+  if ((rc = make_plan(&cfg, B, T, &pl, sc != nullptr))) return rc;
   if (!probs && T > 0) return fail(CTCDEC_E_INVALID, "probs is NULL");
   if (!n_results || !flags) return fail(CTCDEC_E_INVALID, "n_results and flags device buffers are required");
   bool any_eos = false;
@@ -1302,6 +1359,10 @@ int ctcdec_decode_stream_device(const void *probs, int dtype, const int32_t *seq
   io.tokens = tokens; io.timesteps = timesteps; io.scores = scores; io.lens = lens; io.n_results = n_results;
   io.flags = flags; io.out_T = out_T;
   if ((rc = stream_chunk_step(cfg, pl, states, B, T, seq_lens, is_eos, io, nullptr, s))) return rc;
+  if (sc && any_eos) {  // the eos streams' reported scores (the other streams' n_results are 0: their rows are skipped)
+    if ((rc = ensure_ngram_on_device(sc, s0->device))) return rc;
+    if ((rc = launch_readout(sc, tokens, lens, n_results, scores, B, cfg.beam_size, out_T, s))) return rc;
+  }
   return record_device_work(states, B, s);
 }
 
@@ -1809,6 +1870,111 @@ int ctcdec_decode_batch_lm_device(const ctcdec_config *cfg, void *scorer, const 
   CU(cudaMemcpyAsync(scores, h_scores.get(), n_bk * 4, cudaMemcpyHostToDevice, s));
   CU(cudaStreamSynchronize(s));
   return check_error_flags(h_flags, B);
+}
+
+int ctcdec_decode_batch_lm_device_async(const ctcdec_config *cfg, void *scorer, const void *input, int dtype,
+                                        const int32_t *seq_lens, int B, int T, int32_t *tokens, int32_t *timesteps,
+                                        float *scores, int32_t *lens, int32_t *n_results, int32_t *flags,
+                                        float *log_probs_out, void *workspace, size_t workspace_bytes, void *stream) {
+  if (!scorer) return fail(CTCDEC_E_INVALID, "scorer is NULL");
+  if (dtype != -1 && dtype != CTCDEC_DTYPE_F32 && dtype != CTCDEC_DTYPE_F16 && dtype != CTCDEC_DTYPE_BF16)
+    return fail(CTCDEC_E_INVALID, "dtype %d is not -1 (probabilities) or one of CTCDEC_DTYPE_F32 / F16 / BF16", dtype);
+  const int kind = dtype == -1 ? IN_F32 : dtype == CTCDEC_DTYPE_F32 ? IN_LOGITS_F32
+                 : dtype == CTCDEC_DTYPE_F16 ? IN_LOGITS_F16 : IN_LOGITS_BF16;
+  Plan pl;
+  LmWorkspace w;
+  int rc = lm_device_plan(cfg, scorer, B, T, &pl, &w);
+  if (rc) return rc;
+  HostScorer *sc = static_cast<HostScorer *>(scorer);
+  if (!sc->ngram)
+    return fail(CTCDEC_E_UNSUPPORTED, "the asynchronous scorer decode takes a scorer from ctcdec_scorer_create_arpa only: "
+                "a hook scorer needs the host during the call (use ctcdec_decode_batch_lm_device)");
+  if (B > 0 && (!n_results || !flags)) return fail(CTCDEC_E_INVALID, "n_results and flags device buffers are required");
+  if (B > 0 && (!scores || !lens || (T > 0 && (!input || !tokens || !timesteps))))
+    return fail(CTCDEC_E_INVALID, "the input or an output pointer is NULL");
+  if ((rc = check_device())) return rc;
+  int device = 0;
+  CU(cudaGetDevice(&device));
+  if (device >= 64) return fail(CTCDEC_E_INVALID, "device %d out of range", device);
+  if (B == 0) return CTCDEC_OK;
+  const size_t need_bytes = w.total + 256;
+  if (!workspace || workspace_bytes < need_bytes)
+    return fail(CTCDEC_E_WORKSPACE, "workspace of %zu bytes given, %zu needed", workspace_bytes, need_bytes);
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  cudaStreamCaptureStatus capturing = cudaStreamCaptureStatusNone;
+  CU(cudaStreamIsCapturing(s, &capturing));
+  std::lock_guard<std::mutex> lock(g_mu[device]);
+  // nothing that allocates, uploads or synchronises may run while the stream is captured: the scorer's tables must be
+  // on this device already (the first decode puts them there)
+  if (capturing != cudaStreamCaptureStatusNone &&
+      !(sc->d_next && sc->device == device && sc->d_ngram && sc->ngram_device == device))
+    return fail(CTCDEC_E_UNSUPPORTED, "the scorer's tables are not on device %d yet: %s", device, kCaptureFirst);
+  struct CaptureGuard {
+    explicit CaptureGuard(bool on) { g_capturing = on; }
+    ~CaptureGuard() { g_capturing = false; }
+  } guard(capturing != cudaStreamCaptureStatusNone);
+  unsigned char *ws = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(workspace) + 255) / 256 * 256);
+  LmBuffers io;
+  io.in = PruneInput{input, kind, kind == IN_F32 ? nullptr : log_probs_out, true};
+  io.seq_lens = seq_lens;
+  io.ws = ws;
+  io.lm_arena = reinterpret_cast<float *>(ws + w.lm_arena);
+  io.dstate = reinterpret_cast<int *>(ws + w.dstate);
+  io.lm_row = sc->is_character_based ? reinterpret_cast<float *>(ws + w.rows) : nullptr;
+  io.lm_hist = reinterpret_cast<int *>(ws + w.hist);
+  io.tokens = tokens; io.timesteps = timesteps; io.scores = scores; io.lens = lens; io.n_results = n_results;
+  io.flags = flags;
+  // (the host lengths only serve the hook scorers' handshake: the ARPA branch of the step reads the device copy)
+  if ((rc = lm_batch_step(cfg, pl, sc, g_cache[device], device, nullptr, B, T, io, s))) return rc;
+  return launch_readout(sc, tokens, lens, n_results, scores, B, cfg->beam_size, T, s);
+}
+
+// Diagnostic: the read-out of [B, K] host rows, on the host (lm_rescore_batch through the scorer's hooks) or by the
+// read-out kernel on `device` (ARPA scorers).
+int ctcdec_scorer_rescore_rows(void *scorer, const int32_t *tokens, const int32_t *lens, const int32_t *n_results,
+                               float *scores, int B, int K, int row_stride, int device) {
+  if (!scorer) return fail(CTCDEC_E_INVALID, "scorer is NULL");
+  if (B < 0 || K < 1 || row_stride < 0) return fail(CTCDEC_E_INVALID, "bad shape B=%d K=%d row_stride=%d", B, K, row_stride);
+  if (B > 0 && (!lens || !n_results || !scores || (row_stride > 0 && !tokens)))
+    return fail(CTCDEC_E_INVALID, "NULL argument");
+  HostScorer *sc = static_cast<HostScorer *>(scorer);
+  const int V = (int)sc->labels.size();
+  for (int b = 0; b < B; ++b)
+    for (int p = 0; p < n_results[b] && p < K; ++p) {
+      const size_t r = (size_t)b * K + p;
+      if (lens[r] < 0 || lens[r] > row_stride)
+        return fail(CTCDEC_E_INVALID, "row (%d, %d): length %d outside [0, %d]", b, p, lens[r], row_stride);
+      for (int i = 0; i < lens[r]; ++i)
+        if (tokens[r * row_stride + i] < 0 || tokens[r * row_stride + i] >= V)
+          return fail(CTCDEC_E_INVALID, "row (%d, %d): label %d outside [0, %d)", b, p, tokens[r * row_stride + i], V);
+    }
+  if (device < 0) {
+    lm_rescore_batch(*sc, B, K, row_stride, n_results, tokens, lens, scores);
+    return CTCDEC_OK;
+  }
+  if (!sc->ngram) return fail(CTCDEC_E_UNSUPPORTED, "the read-out kernel takes a scorer from ctcdec_scorer_create_arpa only");
+  if (device >= 64) return fail(CTCDEC_E_INVALID, "device %d out of range", device);
+  if (cudaSetDevice(device) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "cudaSetDevice(%d) failed", device);
+  int rc = check_device();
+  if (rc) return rc;
+  if (B == 0) return CTCDEC_OK;
+  std::lock_guard<std::mutex> lock(g_mu[device]);
+  if ((rc = ensure_ngram_on_device(sc, device))) return rc;
+  const size_t rows = (size_t)B * K, tok_bytes = rows * row_stride * 4;
+  unsigned char *d = nullptr;
+  const size_t o_lens = al256(tok_bytes), o_nres = o_lens + al256(rows * 4), o_sc = o_nres + al256((size_t)B * 4);
+  CU(cudaMalloc(&d, o_sc + rows * 4));
+  std::unique_ptr<unsigned char, decltype(&cudaFree)> hold(d, &cudaFree);
+  if (tok_bytes) CU(cudaMemcpy(d, tokens, tok_bytes, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(d + o_lens, lens, rows * 4, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(d + o_nres, n_results, (size_t)B * 4, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(d + o_sc, scores, rows * 4, cudaMemcpyHostToDevice));
+  if ((rc = launch_readout(sc, reinterpret_cast<int32_t *>(d), reinterpret_cast<int32_t *>(d + o_lens),
+                           reinterpret_cast<int32_t *>(d + o_nres), reinterpret_cast<float *>(d + o_sc), B, K,
+                           row_stride, nullptr)))
+    return rc;
+  CU(cudaMemcpy(scores, d + o_sc, rows * 4, cudaMemcpyDeviceToHost));
+  return CTCDEC_OK;
 }
 
 int ctcdec_rows_to_host(const int32_t *d_tokens, const int32_t *d_timesteps, long long rows, int row_stride, int max_len,

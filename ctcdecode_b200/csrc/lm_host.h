@@ -149,6 +149,7 @@ struct HostScorer {
   void *d_ngram = nullptr;
   int ngram_device = -1;
   NgramView d_view;
+  NgramFront d_front;  // the label-to-word front end's tables on the device (the read-out kernel)
   int *d_word_of_state = nullptr, *d_label_word = nullptr;
   // device copies of the dictionary (CUDA library only)
   int *d_next = nullptr;
@@ -312,17 +313,9 @@ static inline void lm_rescore(const HostScorer &sc, int n_results, int row_strid
   for (int p = 0; p < n_results; ++p) {
     const int len = lens[p];
     const int *tok = tokens + (size_t)p * row_stride;
-    float ext = -scores[p];  // scores[prefix] = prefix->score
-    if (!sc.is_character_based && len > 0 && tok[len - 1] != sc.space_id) {  // :173-185 score the last (unfinished) word
-      float s = (float)(cond_rows[p] * sc.alpha);
-      s = (float)((double)s + sc.beta);
-      ext = ext + s;
-    }
-    double approx = (double)ext;  // :194-205
-    approx = approx - (double)len * sc.beta;
-    approx -= sc.hooks.sent_log_prob(sc.hooks.ctx, tok, len) * sc.alpha;
-    const float approx_f = (float)approx;
-    scores[p] = (float)(-(double)approx_f);  // decoder_utils.cpp:68, binding.cpp:91
+    const bool last_word = !sc.is_character_based && len > 0 && tok[len - 1] != sc.space_id;  // :173-185
+    scores[p] = lm_readout_score(scores[p], len, last_word, cond_rows[p], sc.hooks.sent_log_prob(sc.hooks.ctx, tok, len),
+                                 sc.alpha, sc.beta);
   }
 }
 

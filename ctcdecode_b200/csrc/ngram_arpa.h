@@ -33,6 +33,11 @@ struct NgramModel {
   std::vector<std::string> labels;
   int space_id = -1;  // the " " label, -1 if none (reference SPACE_ID_)
   int is_character_based = 1;
+  // the label-to-word front end's tables (ngram_build_front; NgramFront)
+  std::vector<unsigned char> label_bytes, word_bytes;
+  std::vector<int32_t> label_off;
+  std::vector<NgramWordSlot> words;
+  int32_t bos_id = 0, eos_id = 0;
 
   NgramView view() const {
     NgramView v;
@@ -47,11 +52,59 @@ struct NgramModel {
     }
     return v;
   }
+  NgramFront front() const {
+    NgramFront f;
+    f.space_id = space_id;
+    f.is_character_based = is_character_based;
+    f.bos = bos_id;
+    f.eos = eos_id;
+    f.label_bytes = label_bytes.data();
+    f.label_off = label_off.data();
+    f.word_bytes = word_bytes.data();
+    f.words = words.data();
+    f.word_mask = (uint32_t)words.size() - 1;
+    return f;
+  }
   int32_t id_of(const std::string &w) const {
     auto it = word_id.find(w);
     return it == word_id.end() ? 0 : it->second;
   }
 };
+
+// The front end's tables of a loaded model with its labels set: the labels' bytes, and every unigram but <unk> (id 0,
+// which is also what a word missing from the table gets) in an open-addressing table keyed by its spelling.
+static inline void ngram_build_front(NgramModel &m) {
+  m.bos_id = m.id_of("<s>");
+  m.eos_id = m.id_of("</s>");
+  m.label_bytes.clear();
+  m.label_off.assign(1, 0);
+  for (const std::string &l : m.labels) {
+    m.label_bytes.insert(m.label_bytes.end(), l.begin(), l.end());
+    m.label_off.push_back((int32_t)m.label_bytes.size());
+  }
+  size_t cap = 2;
+  while (cap < 2 * m.vocabulary.size()) cap <<= 1;
+  NgramWordSlot empty;
+  empty.hash = empty.off = 0;
+  empty.len = -1;
+  empty.id = 0;
+  m.words.assign(cap, empty);
+  m.word_bytes.clear();
+  const uint32_t mask = (uint32_t)cap - 1;
+  for (size_t id = 1; id < m.vocabulary.size(); ++id) {
+    const std::string &w = m.vocabulary[id];
+    NgramWordSlot e;
+    e.hash = kNgramFnvBasis;
+    for (char c : w) e.hash = ngram_fnv(e.hash, (unsigned char)c);
+    e.off = (uint32_t)m.word_bytes.size();
+    e.len = (int32_t)w.size();
+    e.id = (int32_t)id;
+    m.word_bytes.insert(m.word_bytes.end(), w.begin(), w.end());
+    uint32_t s = e.hash & mask;
+    while (m.words[s].len >= 0) s = (s + 1) & mask;
+    m.words[s] = e;
+  }
+}
 
 namespace arpa_detail {
 
@@ -283,84 +336,20 @@ static inline std::string load_arpa(const char *path, NgramModel &m) {
     for (char c : w) chars += ((c & 0xc0) != 0x80);
     if (chars > 1) m.is_character_based = 0;
   }
+  ngram_build_front(m);
   return "";
 }
 
-// ---- the two hooks: the reference's label-to-word front end (scorer.cpp:95-194) over the lookup ----
-
-// Scorer::make_ngram of the prefix spelled by labels[0..n): the last max_order words (characters for a
-// character-based model), "<s>"-padded in front when the prefix has fewer.
-static inline void ngram_words_of_prefix(const NgramModel &m, const int32_t *labels, int n, std::vector<int32_t> &ids) {
-  std::vector<int32_t> rev;
-  std::string w;
-  int i = n;
-  const int32_t bos = m.id_of("<s>");
-  for (int o = 0; o < m.order; ++o) {
-    w.clear();
-    int j;
-    if (m.is_character_based) {
-      j = i > 0 ? i - 1 : 0;
-      if (i > 0) w = m.labels[labels[j]];
-    } else {
-      j = i;
-      while (j > 0 && labels[j - 1] != m.space_id) --j;
-      for (int k = j; k < i; ++k) w += m.labels[labels[k]];
-    }
-    rev.push_back(m.id_of(w));
-    if (j == 0) {
-      for (int k = 0; k < m.order - o - 1; ++k) rev.push_back(bos);
-      break;
-    }
-    i = m.is_character_based ? j : j - 1;
-  }
-  ids.assign(rev.rbegin(), rev.rend());
-}
+// ---- the two hooks: the front end of ngram_lm.h over the host tables ----
 
 static inline double ngram_hook_cond(void *ctx, const int32_t *labels, int n) {
   const NgramModel &m = *static_cast<const NgramModel *>(ctx);
-  std::vector<int32_t> ids;
-  ngram_words_of_prefix(m, labels, n, ids);
-  return ngram_cond_ids(m.view(), ids.data(), (int)ids.size());
+  return ngram_prefix_cond(m.view(), m.front(), labels, n);
 }
 
-// Scorer::get_sent_log_prob(split_labels(prefix)): "<s>"-padded sentence + "</s>", every max_order window scored from
-// the null context, summed in double.
 static inline double ngram_hook_sent(void *ctx, const int32_t *labels, int n) {
   const NgramModel &m = *static_cast<const NgramModel *>(ctx);
-  std::string s;
-  for (int i = 0; i < n; ++i) s += m.labels[labels[i]];
-  std::vector<int32_t> sent;
-  const int32_t bos = m.id_of("<s>");
-  const size_t order = (size_t)m.order;
-  std::vector<std::string> words;
-  if (n > 0) {
-    if (m.is_character_based) {
-      std::string cur;  // split_utf8_str (decoder_utils.cpp:83-100)
-      for (char c : s) {
-        if ((c & 0xc0) != 0x80 && !cur.empty()) { words.push_back(cur); cur.clear(); }
-        cur.push_back(c);
-      }
-      words.push_back(cur);
-    } else {
-      size_t start = 0;  // split_str(s, " ") (decoder_utils.cpp:102-120)
-      while (true) {
-        const size_t end = s.find(' ', start);
-        if (end == std::string::npos) {
-          if (start < s.size()) words.push_back(s.substr(start));
-          break;
-        }
-        if (end > start) words.push_back(s.substr(start, end - start));
-        start = end + 1;
-      }
-    }
-  }
-  sent.assign(words.empty() ? order : order - 1, bos);
-  for (const std::string &w : words) sent.push_back(m.id_of(w));
-  sent.push_back(m.id_of("</s>"));
-  const NgramView v = m.view();
-  double score = 0.0;
-  for (size_t i = 0; i + order <= sent.size(); ++i) score += ngram_cond_ids(v, sent.data() + i, (int)order);
-  return score;
+  return ngram_sentence(m.view(), m.front(), labels, n);
 }
 
 }  // namespace ctc

@@ -1,7 +1,8 @@
-// N-gram language model read from an ARPA text file: the tables, and the one lookup that reproduces the reference's
-// Scorer::get_log_cond_prob (scorer.cpp:74-93) over KenLM's probing model bit for bit.  The tables and the lookup
-// compile for the host and for the device (ngram_cond_ids takes plain pointers: a view of host vectors or of their
-// HBM copies); the ARPA loader and the label-to-word front end are host code.
+// N-gram language model read from an ARPA text file: the tables, the one lookup that reproduces the reference's
+// Scorer::get_log_cond_prob (scorer.cpp:74-93) over KenLM's probing model bit for bit, the reference's label-to-word
+// front end (make_ngram, split_labels, get_sent_log_prob) and the read-out rescoring of a result row.  All of it
+// compiles for the host and for the device (plain pointers: views of host vectors or of their HBM copies); the ARPA
+// loader and the building of the tables are host code (ngram_arpa.h).
 //
 // What is reproduced, from KenLM's query path (lm/model.cc FullScore / ResumeScore, lm/read_arpa.cc):
 //   * word ids: 0 is <unk> (also "<UNK>"), then the unigrams in file order; an unknown string is 0;
@@ -121,6 +122,191 @@ CTC_NG_HD double ngram_cond_ids(const NgramView &m, const int32_t *ids, int n) {
   return (double)p / (double)kNgramFltLogE;
 }
 
+// ---- the reference's label-to-word front end (scorer.cpp:95-194, decoder_utils.cpp:83-120) over flat tables ----
+
+// One unigram of the spelling table (open addressing); len < 0 marks an empty slot.
+struct NgramWordSlot {
+  uint32_t hash, off;  // FNV-1a of the spelling, its offset in the spelling bytes
+  int32_t len, id;     // spelling length in bytes, KenLM word id
+};
+
+// Read-only view of the front end's tables, built once per model (ngram_build_front): the decoder's labels as one byte
+// blob, and a lookup from a word's bytes to its id (0 for a word the model does not have, as KenLM's index()).
+struct NgramFront {
+  int space_id = -1;            // the " " label, -1 if none
+  int is_character_based = 1;
+  int32_t bos = 0, eos = 0;     // ids of "<s>" / "</s>"
+  const unsigned char *label_bytes = nullptr;  // label l: label_bytes[label_off[l] .. label_off[l + 1])
+  const int32_t *label_off = nullptr;          // [labels + 1]
+  const unsigned char *word_bytes = nullptr;   // the unigrams' spellings
+  const NgramWordSlot *words = nullptr;        // [word_mask + 1], a power of two at least twice the unigram count
+  uint32_t word_mask = 0;
+};
+
+CTC_NG_HD uint32_t ngram_fnv(uint32_t h, unsigned char c) { return (h ^ c) * 16777619u; }
+constexpr uint32_t kNgramFnvBasis = 2166136261u;
+
+// A byte position in the string a label row spells: byte o of label tok[k]; k == n is the end.  Positions are kept
+// normalised (o inside its label, empty labels skipped), so two equal positions compare equal.
+struct NgramPos { int k, o; };
+
+CTC_NG_HD int ngram_label_len(const NgramFront &f, int32_t l) { return f.label_off[l + 1] - f.label_off[l]; }
+CTC_NG_HD NgramPos ngram_norm(const NgramFront &f, const int32_t *tok, int n, NgramPos c) {
+  while (c.k < n && c.o >= ngram_label_len(f, tok[c.k])) { ++c.k; c.o = 0; }
+  return c;
+}
+CTC_NG_HD unsigned char ngram_byte(const NgramFront &f, const int32_t *tok, NgramPos c) {
+  return f.label_bytes[f.label_off[tok[c.k]] + c.o];
+}
+CTC_NG_HD NgramPos ngram_next(const NgramFront &f, const int32_t *tok, int n, NgramPos c) {
+  ++c.o;
+  return ngram_norm(f, tok, n, c);
+}
+CTC_NG_HD bool ngram_same(NgramPos a, NgramPos b) { return a.k == b.k && a.o == b.o; }
+
+// The id of the word spelled by the bytes [a, b) of the row (Scorer's ext_scorer index(), 0 if the model lacks it).
+// The bytes are walked twice, once for the hash and once per candidate, so no word buffer is needed.
+CTC_NG_HD int32_t ngram_word_id(const NgramFront &f, const int32_t *tok, int n, NgramPos a, NgramPos b) {
+  uint32_t h = kNgramFnvBasis;
+  int32_t len = 0;
+  for (NgramPos c = a; !ngram_same(c, b); c = ngram_next(f, tok, n, c)) {
+    h = ngram_fnv(h, ngram_byte(f, tok, c));
+    ++len;
+  }
+  for (uint32_t s = h & f.word_mask;; s = (s + 1) & f.word_mask) {
+    const NgramWordSlot &w = f.words[s];
+    if (w.len < 0) return 0;
+    if (w.hash != h || w.len != len) continue;
+    NgramPos c = a;
+    int32_t i = 0;
+    for (; i < len && ngram_byte(f, tok, c) == f.word_bytes[w.off + i]; ++i) c = ngram_next(f, tok, n, c);
+    if (i == len) return w.id;
+  }
+}
+
+// Scorer::get_log_cond_prob(Scorer::make_ngram(prefix)) of the prefix spelled by tok[0..n): the last max_order words
+// (split on the space label; one label per word for a character-based model), "<s>"-padded in front when the prefix has
+// fewer.
+CTC_NG_HD double ngram_prefix_cond(const NgramView &m, const NgramFront &f, const int32_t *tok, int n) {
+  int32_t ids[kNgramMaxOrder];
+  int got = 0, i = n;
+  for (int o = 0; o < m.order; ++o) {
+    int j;
+    if (f.is_character_based) {
+      j = i > 0 ? i - 1 : 0;
+    } else {
+      j = i;
+      while (j > 0 && tok[j - 1] != f.space_id) --j;
+    }
+    // the word is labels [j, i); a character-based model's is the one label i - 1 (none at the start)
+    const NgramPos a = ngram_norm(f, tok, n, NgramPos{j, 0}), b = ngram_norm(f, tok, n, NgramPos{i, 0});
+    ids[m.order - 1 - got++] = ngram_word_id(f, tok, n, a, b);
+    if (j == 0) {
+      for (int k = 0; k < m.order - o - 1; ++k) ids[m.order - 1 - got++] = m.bos;
+      break;
+    }
+    i = f.is_character_based ? j : j - 1;
+  }
+  return ngram_cond_ids(m, ids + m.order - got, got);
+}
+
+// Scorer::get_sent_log_prob(Scorer::split_labels(prefix)) of tok[0..n): the labels' concatenated string split on ' '
+// bytes with split_str's rule (empty pieces dropped), or into UTF-8 characters for a character-based model
+// (split_utf8_str); "<s>"-padded, "</s>" appended, every max_order window scored from the null context and summed in
+// double from left to right.  The sentence is streamed through a window of max_order ids.
+CTC_NG_HD double ngram_sentence(const NgramView &m, const NgramFront &f, const int32_t *tok, int n) {
+  const NgramPos end{n, 0};
+  NgramPos c = ngram_norm(f, tok, n, NgramPos{0, 0});
+  bool any_word = n > 0;  // split_utf8_str gives one word, possibly empty, for any non-empty prefix
+  if (!f.is_character_based) {
+    any_word = false;
+    for (NgramPos q = c; !ngram_same(q, end) && !any_word; q = ngram_next(f, tok, n, q)) any_word = ngram_byte(f, tok, q) != ' ';
+  }
+  int pads = any_word ? m.order - 1 : m.order;
+  bool empty_word = f.is_character_based && n > 0 && ngram_same(c, end), eos_done = false;
+  int32_t win[kNgramMaxOrder];  // the last max_order ids of the sentence so far
+  int cnt = 0;
+  double score = 0.0;
+  while (true) {  // one id of the sentence per pass (one inlined lookup for the whole sentence)
+    int32_t id;
+    if (pads > 0) {
+      id = m.bos;
+      --pads;
+    } else if (empty_word) {
+      id = ngram_word_id(f, tok, n, c, c);
+      empty_word = false;
+    } else {
+      if (!f.is_character_based)
+        while (!ngram_same(c, end) && ngram_byte(f, tok, c) == ' ') c = ngram_next(f, tok, n, c);
+      if (!ngram_same(c, end)) {
+        const NgramPos a = c;
+        c = ngram_next(f, tok, n, c);
+        if (f.is_character_based)
+          while (!ngram_same(c, end) && (ngram_byte(f, tok, c) & 0xc0) == 0x80) c = ngram_next(f, tok, n, c);
+        else
+          while (!ngram_same(c, end) && ngram_byte(f, tok, c) != ' ') c = ngram_next(f, tok, n, c);
+        id = ngram_word_id(f, tok, n, a, c);
+      } else if (!eos_done) {
+        id = f.eos;
+        eos_done = true;
+      } else {
+        break;
+      }
+    }
+    if (cnt == m.order) {
+      for (int k = 1; k < m.order; ++k) win[k - 1] = win[k];
+      win[m.order - 1] = id;
+    } else {
+      win[cnt++] = id;
+    }
+    if (cnt == m.order) score += ngram_cond_ids(m, win, m.order);
+  }
+  return score;
+}
+
+// ---- the read-out rescoring (reference DecoderState::decode, ctc_beam_search_decoder.cpp:173-208) ----
+// Every double operation rounds as in the x86-64 host build, which has no FMA: on the device the multiplies, adds and
+// subtracts are written as _rn intrinsics, which nvcc never contracts.
+#if defined(__CUDA_ARCH__)
+#define CTC_NG_DMUL(a, b) __dmul_rn((a), (b))
+#define CTC_NG_DADD(a, b) __dadd_rn((a), (b))
+#define CTC_NG_DSUB(a, b) __dsub_rn((a), (b))
+#else
+#define CTC_NG_DMUL(a, b) ((a) * (b))
+#define CTC_NG_DADD(a, b) ((a) + (b))
+#define CTC_NG_DSUB(a, b) ((a) - (b))
+#endif
+
+// The reported score of one result row.  score: what the finalize kernel wrote (minus the raw prefix score); len: the
+// row's length; last_word: a word-based row whose last label is not the space, so that its unfinished last word is
+// scored: float(cond * alpha), then float(s + beta) added to the raw score in float.  Then approx_ctc =
+// double(raw) - len * beta - sent * alpha, reported as -double(float(approx_ctc)) (decoder_utils.cpp:68, binding.cpp:91).
+CTC_NG_HD float lm_readout_score(float score, int len, bool last_word, double cond, double sent, double alpha,
+                                 double beta) {
+  float ext = -score;
+  if (last_word) {
+    float s = (float)CTC_NG_DMUL(cond, alpha);
+    s = (float)CTC_NG_DADD((double)s, beta);
+    ext = ext + s;
+  }
+  double approx = (double)ext;
+  approx = CTC_NG_DSUB(approx, CTC_NG_DMUL((double)len, beta));
+  approx = CTC_NG_DSUB(approx, CTC_NG_DMUL(sent, alpha));
+  const float approx_f = (float)approx;
+  return (float)(-(double)approx_f);
+}
+
+// lm_readout_score of the row tok[0..len) with an ARPA model: both terms from the front end above.
+CTC_NG_HD float ngram_readout_row(const NgramView &m, const NgramFront &f, const int32_t *tok, int len, float score,
+                                  double alpha, double beta) {
+  const bool last_word = !f.is_character_based && len > 0 && tok[len - 1] != f.space_id;
+  const double cond = last_word ? ngram_prefix_cond(m, f, tok, len) : 0.0;
+  return lm_readout_score(score, len, last_word, cond, ngram_sentence(m, f, tok, len), alpha, beta);
+}
+
 }  // namespace ctc
 
+#undef CTC_NG_DMUL
+#undef CTC_NG_DADD
+#undef CTC_NG_DSUB
 #undef CTC_NG_HD

@@ -21,10 +21,18 @@ Differences from the reference, all additive:
     because the host answers the beam kernel's per-frame LM handshake while it runs.  The online decoder takes a
     scorer too (device-resident states, one persistent launch per chunk).  Character-based models are detected like
     the reference does (every word of the model is one UTF-8 character) and decoded without a dictionary.
+  * ``non_blocking=True`` (with ``device_outputs=True``, and ``scorer_provider="device"`` when there is a language
+    model): a CUDA decode with the device scorer is only enqueued on the current stream, read-out rescoring included
+    (ctcdec_decode_batch_lm_device_async / ctcdec_decode_stream_device), so it can run behind the acoustic model and
+    be captured into a CUDA graph (decode once before capturing; a graph replays the alpha / beta it captured).  The
+    call may return before the results exist, and a kernel error shows only as CTCDEC_FLAG_ERR_ARENA in
+    ``last_flags``, a CUDA tensor.  ``OnlineCTCBeamDecoder`` then decodes CUDA chunks and ``decode_logits`` with the
+    device scorer on the GPU as well.
   * the [batch, beam, T] result tensors are PAGE-LOCKED CPU tensors (torch's caching host allocator, so a decode loop
     reuses the same blocks) up to CTCDECODE_B200_PIN_OUTPUT_BYTES per tensor (default 1 GiB), pageable beyond: a fresh
     pageable [256, 100, 1000] int32 pair costs page faults on every call, several times the decode itself.
-  * ``OnlineCTCBeamDecoder``: CUDA chunks (without a scorer) are decoded in place on the current stream, raw logits go
+  * ``OnlineCTCBeamDecoder``: CUDA chunks (without a scorer, or with ``non_blocking=True``) are decoded in place on the
+    current stream, raw logits go
     through ``decode_logits``, ``device_outputs=True`` leaves the results on the GPU, and ``committed_prefix`` reports
     the part of each stream's transcript no later chunk can change.
   * ``device="all"`` (or no device and a CPU batch of more than 4 x 132 utterances on a multi-GPU box): the host batch
@@ -68,7 +76,14 @@ def _cfg(decoder):
 
 class _Base(object):
     def _init_common(self, labels, model_path, alpha, beta, cutoff_top_n, cutoff_prob, beam_width, num_processes,
-                     blank_id, log_probs_input, device, scorer_provider=None):
+                     blank_id, log_probs_input, device, scorer_provider=None, non_blocking=False):
+        if non_blocking and not self._device_outputs:
+            raise ValueError("non_blocking=True needs device_outputs=True: the results stay on the GPU")
+        if non_blocking and model_path and \
+                (scorer_provider or os.environ.get("CTCDECODE_B200_SCORER_PROVIDER")) != "device":
+            raise ValueError('non_blocking=True with a language model needs scorer_provider="device": a hook scorer '
+                             "answers the decode on the host")
+        self._non_blocking = bool(non_blocking)
         self._beam_width = int(beam_width)
         self._scorer = None
         self._num_processes = num_processes
@@ -114,12 +129,12 @@ class CTCBeamDecoder(_Base):
 
     def __init__(self, labels, model_path=None, alpha=0, beta=0, cutoff_top_n=40, cutoff_prob=1.0, beam_width=100,
                  num_processes=4, blank_id=0, log_probs_input=False, device=None, device_outputs=False,
-                 scorer_provider=None):
+                 scorer_provider=None, non_blocking=False):
         self.cutoff_top_n = cutoff_top_n  # public attribute name kept from the reference (:39)
         self._device_outputs = device_outputs
         self._ws = None
         self._init_common(labels, model_path, alpha, beta, cutoff_top_n, cutoff_prob, beam_width, num_processes,
-                          blank_id, log_probs_input, device, scorer_provider)
+                          blank_id, log_probs_input, device, scorer_provider, non_blocking)
 
     def _cutoff_top_n_value(self):
         return int(self.cutoff_top_n)
@@ -222,9 +237,10 @@ class CTCBeamDecoder(_Base):
         scorer = self._scorer.handle if self._scorer is not None else None
         if logits_dtype is None:
             probs = probs.float().contiguous()
+        lm_async = scorer and self._non_blocking
         if seq_lens is not None:
-            # (the scorer path answers every utterance's per-frame handshake on the host: its lengths stay there)
-            seq_lens = seq_lens.to(device="cpu" if scorer else dev, dtype=torch.int32).contiguous()
+            # (the blocking scorer path answers every utterance's per-frame handshake on the host: its lengths stay there)
+            seq_lens = seq_lens.to(device="cpu" if scorer and not lm_async else dev, dtype=torch.int32).contiguous()
         nbytes = ctypes.c_size_t(0)
         if scorer:
             _native.check(lib.ctcdec_lm_workspace_bytes(ctypes.byref(cfg), scorer, B, T, ctypes.byref(nbytes)))
@@ -241,8 +257,11 @@ class CTCBeamDecoder(_Base):
         flags = torch.zeros(B, dtype=torch.int32, device=dev)
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev).cuda_stream
-            if scorer:  # (returns when the results are in place: the host serves the LM during the call)
-                _native.check(lib.ctcdec_decode_batch_lm_device(
+            if scorer:
+                # blocking: returns when the results are in place (the host serves a hook scorer during the call and
+                # rescores the results); non_blocking: enqueued on the stream, read-out included
+                fn = lib.ctcdec_decode_batch_lm_device_async if lm_async else lib.ctcdec_decode_batch_lm_device
+                _native.check(fn(
                     ctypes.byref(cfg), scorer, probs.data_ptr(), -1 if logits_dtype is None else logits_dtype,
                     seq_lens.data_ptr() if seq_lens is not None else None, B, T, output.data_ptr(),
                     timesteps.data_ptr(), scores.data_ptr(), out_seq_len.data_ptr(), n_results.data_ptr(),
@@ -287,12 +306,13 @@ class OnlineCTCBeamDecoder(_Base):
 
     def __init__(self, labels, model_path=None, alpha=0, beta=0, cutoff_top_n=40, cutoff_prob=1.0, beam_width=100,
                  num_processes=4, blank_id=0, log_probs_input=False, device=None, scorer_provider=None,
-                 device_outputs=False):
+                 device_outputs=False, non_blocking=False):
         self._cutoff_top_n = cutoff_top_n  # private name kept from the reference (:175)
         self._device_outputs = device_outputs
         self._ws = None
         self._init_common(labels, model_path, alpha, beta, cutoff_top_n, cutoff_prob, beam_width, num_processes,
-                          blank_id, log_probs_input, device, scorer_provider=scorer_provider)
+                          blank_id, log_probs_input, device, scorer_provider=scorer_provider,
+                          non_blocking=non_blocking)
 
     def _cutoff_top_n_value(self):
         return int(self._cutoff_top_n)
@@ -302,14 +322,15 @@ class OnlineCTCBeamDecoder(_Base):
         __init__.py:189-238: beam_results / timesteps are [B, n_beams, max_len] (both [B, 0, 0] while no stream
         has reached eos), beam_scores / out_lens are [B, beam].
 
-        A CUDA chunk (without a scorer) is decoded in place on the current stream (ctcdec_decode_stream_device).
+        A CUDA chunk (without a scorer, or with non_blocking=True) is decoded in place on the current stream
+        (ctcdec_decode_stream_device).
         With device_outputs=True the results stay on the GPU and the call does not wait for it: beam_results /
         timesteps are [B, beam, out_T] (out_T: the most frames an eos stream has consumed; [B, 0, 0] without eos),
         only [b, p, :out_lens[b, p]] of rows p < last_n_results[b] of eos streams being meaningful."""
         lib = _native.load()
         if probs.dim() != 3:
             raise ValueError("probs must be [batch, time, labels], got %s" % (tuple(probs.shape),))
-        if probs.is_cuda and self._scorer is None:
+        if probs.is_cuda and (self._scorer is None or self._non_blocking):
             return self._decode_device(lib, probs, states, is_eos_s, seq_lens, -1)
         probs = probs.cpu().float().contiguous()
         B, T, V = probs.shape
@@ -353,8 +374,9 @@ class OnlineCTCBeamDecoder(_Base):
         float16 / bfloat16; each frame's float32 log-softmax is taken on the fly (as CTCBeamDecoder.decode_logits
         does), so chunks decode exactly like the concatenated logits would offline."""
         lib = _native.load()
-        if self._scorer is not None:
-            raise NotImplementedError("ctcdecode_b200: decode_logits with a scorer is not built")
+        if self._scorer is not None and not self._non_blocking:
+            raise NotImplementedError("ctcdecode_b200: decode_logits with a scorer needs non_blocking=True "
+                                      "(and scorer_provider=\"device\")")
         if logits.dim() != 3 or not logits.is_cuda:
             raise ValueError("logits must be a CUDA tensor [batch, time, labels]")
         dtypes = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}

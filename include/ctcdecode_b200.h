@@ -179,7 +179,9 @@ int ctcdec_scorer_create(const ctcdec_scorer_hooks *hooks, double alpha, double 
  * device once per device, and the beam kernel computes the LM terms of the trie nodes it creates itself: the offline
  * entries and ctcdec_decode_stream_host run without the per-frame host handshake (one launch per batch or chunk), and
  * the device keeps the last max_order - 1 word ids of every node, batch x (1 + beam x frames) x (max_order - 1) x 4
- * bytes (CTCDEC_E_UNSUPPORTED beyond 64 GiB).  The read-out rescoring stays on the host, through this scorer's hooks.
+ * bytes (CTCDEC_E_UNSUPPORTED beyond 64 GiB).  The blocking entries rescore their results on the host, through this
+ * scorer's hooks; ctcdec_decode_batch_lm_device_async and ctcdec_decode_stream_device rescore them on the device with
+ * the same label-to-word front end over tables of the labels' bytes and the unigrams' spellings.
  * Refused with CTCDEC_E_UNSUPPORTED, the reason in ctcdec_last_error(), anything the tables cannot reproduce exactly:
  * a KenLM binary file or other non-ARPA input, order 1 or above 6, counts that disagree with the sections, a malformed
  * line, a duplicate entry, an n-gram word missing from the unigrams, no <s> or </s>, an n-gram whose context or suffix
@@ -191,6 +193,14 @@ int ctcdec_scorer_create_arpa(const char *path, double alpha, double beta, const
  * hook scorer or an ARPA scorer.  Labels must lie in [0, n_labels). */
 int ctcdec_scorer_cond_log_prob(const void *scorer, const int32_t *labels, int n, double *out);
 int ctcdec_scorer_sent_log_prob(const void *scorer, const int32_t *labels, int n, double *out);
+/* Diagnostic: the read-out rescoring of [B, K] result rows in HOST buffers, as the decodes apply it (reference
+ * DecoderState::decode, ctc_beam_search_decoder.cpp:173-208).  tokens [B, K, row_stride], lens [B, K], n_results [B]:
+ * rows p < min(n_results[b], K) are rescored in scores [B, K] (which hold minus the raw prefix scores, as the finalize
+ * kernel writes them), the others are left alone.  device < 0: on the host, through the scorer's hooks (any scorer);
+ * device >= 0: by the read-out kernel on that device (a scorer from ctcdec_scorer_create_arpa only, else
+ * CTCDEC_E_UNSUPPORTED).  Labels must lie in [0, n_labels) and lengths in [0, row_stride]. */
+int ctcdec_scorer_rescore_rows(void *scorer, const int32_t *tokens, const int32_t *lens, const int32_t *n_results,
+                               float *scores, int B, int K, int row_stride, int device);
 /* Replaces: paddle_release_scorer, is_character_based, get_max_order, get_dict_size, reset_params
  * (binding.cpp:267-287). */
 int ctcdec_scorer_destroy(void *scorer);
@@ -239,6 +249,28 @@ int ctcdec_decode_batch_lm_device(const ctcdec_config *cfg, void *scorer, const 
                                   float *scores, int32_t *lens, int32_t *n_results, int32_t *flags,
                                   float *log_probs_out, void *workspace, size_t workspace_bytes, void *stream);
 
+/* ctcdec_decode_batch_lm_device for a scorer from ctcdec_scorer_create_arpa, WITHOUT waiting: the same arguments, outputs
+ * and workspace (ctcdec_lm_workspace_bytes), except that seq_lens is a DEVICE int32 [B] buffer (or NULL).  The prune,
+ * beam and finalize kernels and the read-out kernel (the reference's approx_ctc rescoring, computed on the device from
+ * the scorer's tables) are enqueued on `stream` after the work already queued there, and the call returns; the results
+ * are in place when the stream gets past them.  After its checks the call allocates nothing, copies nothing to or
+ * from pageable or pinned host memory and never synchronises, except on its first use of a scorer on a device, which
+ * uploads the scorer's tables and raises the kernels' shared-memory limits.
+ *   CUDA graphs: the call can be captured.  Decode once outside the capture first (same scorer, device and shapes): a
+ *              call made during capture that would have to upload the tables or raise a kernel's limit returns
+ *              CTCDEC_E_UNSUPPORTED instead; the capture stays valid (a refusal over a kernel's limit may leave part of
+ *              the decode in the graph, which the caller then discards).  alpha and beta are read when the work is
+ *              enqueued, so a graph replays the values it captured: capture again after ctcdec_scorer_reset_params.
+ *   Errors of the kernels show in flags only: a set CTCDEC_FLAG_ERR_ARENA means the utterance's results are not valid
+ *              (as with ctcdec_decode_stream_device).
+ * A hook scorer returns CTCDEC_E_UNSUPPORTED (its language model runs on the host during the decode: use
+ * ctcdec_decode_batch_lm_device).  The workspace and outputs must not be reused before the stream has finished with
+ * them.  Enqueueing on one device serialises, the kernels of different streams overlap. */
+int ctcdec_decode_batch_lm_device_async(const ctcdec_config *cfg, void *scorer, const void *input, int dtype,
+                                        const int32_t *seq_lens, int B, int T, int32_t *tokens, int32_t *timesteps,
+                                        float *scores, int32_t *lens, int32_t *n_results, int32_t *flags,
+                                        float *log_probs_out, void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---- streaming (OnlineCTCBeamDecoder) ------------------------------------------------------------- */
 
 /* Replaces: paddle_get_decoder_state (binding.cpp:246-261).  The state (beam + trie + absolute frame
@@ -284,8 +316,11 @@ int ctcdec_stream_workspace_bytes(const ctcdec_config *cfg, int B, int T, size_t
  *              code without waiting for the kernels.
  * The call does not wait for the device, with one exception: when a stream's node arena must grow (1 + beam x frames
  * nodes, capacity doubling from 256 frames: about log2(frames / 256) times per stream) the old arena is copied on
- * `stream` and the host waits for that copy before freeing it.  States with a scorer return CTCDEC_E_UNSUPPORTED
- * (their beam kernel needs the per-frame host handshake of ctcdec_decode_stream_host).  The workspace and the outputs
+ * `stream` and the host waits for that copy before freeing it.  States with a scorer from ctcdec_scorer_create_arpa are
+ * decoded here too (the first call uploads the scorer's tables): the beam kernel computes the LM terms, and at eos the
+ * read-out kernel rescores the eos streams' rows on the device (alpha and beta as they are when the call is made).
+ * States with a hook scorer return CTCDEC_E_UNSUPPORTED (their beam kernel needs the per-frame host handshake of
+ * ctcdec_decode_stream_host).  The workspace and the outputs
  * must not be reused before the work on `stream` is done, as with ctcdec_decode_batch_device.
  * Device-path calls record an event on each state; ctcdec_decode_stream_host waits for it on its own stream, a later
  * device-path call on another stream waits for it too, and ctcdec_state_destroy synchronises it before freeing. */

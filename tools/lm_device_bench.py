@@ -6,7 +6,7 @@ beta 1.0) through CTCBeamDecoder three ways:
   device          CUDA probabilities through the device entry point (ctcdec_decode_batch_lm_device)
   logits_f16      decode_logits of fp16 logits (the device entry, the log-softmax taken by the scan kernel)
 
-    python tools/lm_device_bench.py [--reps N] [--device I] [--scorer hook|device]
+    python tools/lm_device_bench.py [--reps N] [--device I] [--scorer hook|device|async]
 
 --scorer device times the library's own ARPA scorer (scorer_provider="device": the beam kernel computes the LM terms,
 no per-frame host handshake) against the hook scorer on the same CUDA probabilities instead:
@@ -15,8 +15,16 @@ no per-frame host handshake) against the hook scorer on the same CUDA probabilit
   ngram           the device scorer, CUDA probabilities (the same entry point)
   ngram_host      the device scorer, CPU probabilities (ctcdec_decode_batch_lm_host)
 
-Every path is warmed up, then timed N times in alternating rounds with a host clock around the call (each call
-returns synchronised, with CPU results).  Prints one JSON line: per path the median and the spread of the call time
+--scorer async times the device scorer with device outputs three ways, on the same CUDA probabilities:
+
+  blocking        ctcdec_decode_batch_lm_device: the call synchronises and rescores the results on the host
+  async           non_blocking=True (ctcdec_decode_batch_lm_device_async): the read-out kernel rescores them
+  graph           the async decode captured once into a CUDA graph, replayed
+
+and, in a separate profiled pass afterwards, the CUDA time of the read-out kernel alone (torch.profiler).
+
+Every path is warmed up, then timed N times in alternating rounds with a host clock around the call and a device
+synchronise after it.  Prints one JSON line: per path the median and the spread of the call time
 and utterances/s; whether the host and device paths gave identical outputs; the card and its power limit, read in the
 same run.  Writes nothing to disk.
 """
@@ -58,8 +66,9 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=5, help="timed calls per path")
     ap.add_argument("--device", type=int, default=0)
-    ap.add_argument("--scorer", choices=["hook", "device"], default="hook",
-                    help="hook: the three input paths of the hook scorer; device: the device scorer against the hook")
+    ap.add_argument("--scorer", choices=["hook", "device", "async"], default="hook",
+                    help="hook: the three input paths of the hook scorer; device: the device scorer against the hook; "
+                         "async: the device scorer's blocking, asynchronous and graph-replayed decodes")
     args = ap.parse_args()
     dev = torch.device("cuda", args.device)
     torch.cuda.set_device(dev)
@@ -68,14 +77,33 @@ def main():
     probs = c5_inputs(B, T, 0)
     probs_d = probs.to(dev)
     logits = probs_d.clamp_min(1e-20).log().mul(1.25).half()
-    dec = CTCBeamDecoder(L29, model_path=TINY_LM, alpha=cfg["alpha"], beta=cfg["beta"], beam_width=cfg["beam"],
-                         cutoff_top_n=cfg["cutoff_top_n"], cutoff_prob=cfg["cutoff_prob"], scorer_provider=PROVIDER)
-    paths = {"host": (dec, lambda: dec.decode(probs)), "device": (dec, lambda: dec.decode(probs_d)),
-             "logits_f16": (dec, lambda: dec.decode_logits(logits))}
-    compared = ("host", "device")
+    kw = dict(model_path=TINY_LM, alpha=cfg["alpha"], beta=cfg["beta"], beam_width=cfg["beam"],
+              cutoff_top_n=cfg["cutoff_top_n"], cutoff_prob=cfg["cutoff_prob"])
+    readout_ms = None
+    if args.scorer == "async":
+        bdec = CTCBeamDecoder(L29, scorer_provider="device", device_outputs=True, **kw)
+        adec = CTCBeamDecoder(L29, scorer_provider="device", device_outputs=True, non_blocking=True, **kw)
+        gdec = CTCBeamDecoder(L29, scorer_provider="device", device_outputs=True, non_blocking=True, **kw)
+        static = probs_d.clone()
+        gdec.decode(static)  # outside the capture first: tables, kernel limits
+        torch.cuda.synchronize(dev)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            g_out = list(gdec.decode(static)) + [gdec.last_n_results, gdec.last_flags]
+
+        def replay():
+            graph.replay()
+            return g_out[:4]
+        paths = {"blocking": (bdec, lambda: bdec.decode(probs_d)), "async": (adec, lambda: adec.decode(probs_d)),
+                 "graph": (gdec, replay)}
+        compared = ("blocking", "async")
+    else:
+        dec = CTCBeamDecoder(L29, scorer_provider=PROVIDER, **kw)
+        paths = {"host": (dec, lambda: dec.decode(probs)), "device": (dec, lambda: dec.decode(probs_d)),
+                 "logits_f16": (dec, lambda: dec.decode_logits(logits))}
+        compared = ("host", "device")
     if args.scorer == "device":
-        ndec = CTCBeamDecoder(L29, model_path=TINY_LM, alpha=cfg["alpha"], beta=cfg["beta"], beam_width=cfg["beam"],
-                              cutoff_top_n=cfg["cutoff_top_n"], cutoff_prob=cfg["cutoff_prob"], scorer_provider="device")
+        ndec = CTCBeamDecoder(L29, scorer_provider="device", **kw)
         paths = {"hook": (dec, lambda: dec.decode(probs_d)), "ngram": (ndec, lambda: ndec.decode(probs_d)),
                  "ngram_host": (ndec, lambda: ndec.decode(probs))}
         compared = ("hook", "ngram")
@@ -86,7 +114,9 @@ def main():
         res = fn()
         torch.cuda.synchronize(dev)
         dt = time.perf_counter() - t0
-        return dt, list(res) + [d.last_n_results.clone(), d.last_flags.clone()]
+        if name == "graph":
+            return dt, [x.cpu() for x in g_out]
+        return dt, [x.cpu() for x in res] + [d.last_n_results.cpu(), d.last_flags.cpu()]
 
     outs, times = {}, {name: [] for name in paths}
     for name in paths:
@@ -101,10 +131,22 @@ def main():
     same = identical(outs[compared[0]], outs[compared[1]])
     if args.scorer == "device":
         same = same and identical(outs["ngram"], outs["ngram_host"])
+    if args.scorer == "async":
+        same = same and identical(outs["async"], outs["graph"])
+        # the read-out kernel alone, from a profiled pass of its own (the timed rounds above run without the profiler)
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(args.reps):
+                adec.decode(probs_d)
+            torch.cuda.synchronize(dev)
+        ks = [e.device_time for e in prof.events() if "lm_readout_kernel" in e.name]
+        readout_ms = {"ms_median": statistics.median(ks) / 1e3, "ms_min": min(ks) / 1e3, "ms_max": max(ks) / 1e3,
+                      "launches": len(ks)} if ks else None
     print(json.dumps({"workload": cfg["name"], "scorer": args.scorer, "card": card_info(args.device), "paths": legs,
-                      "%s_%s_identical" % compared: bool(same),
-                      "note": "host clock around each call, which returns synchronised with CPU results; paths "
-                              "alternate within each round"}), flush=True)
+                      "readout_kernel": readout_ms,
+                      ("all_arms_identical" if args.scorer == "async" else "%s_%s_identical" % compared): bool(same),
+                      "note": "host clock around each call and a device synchronise after it; paths alternate within "
+                              "each round"}), flush=True)
     assert same, "%s and %s gave different results" % compared
 
 
