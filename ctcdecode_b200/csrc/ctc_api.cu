@@ -482,7 +482,8 @@ static int ensure_dict_on_device(HostScorer *sc, int device) {
   return CTCDEC_OK;
 }
 
-// The tables of an ARPA scorer and the kernel's word-id arrays in device memory, uploaded once per device.
+// The tables of an n-gram scorer (ARPA or KenLM binary) and the kernel's word-id arrays in device memory, uploaded once
+// per device.
 static int ensure_ngram_on_device(HostScorer *sc, int device) {
   if (sc->d_ngram && sc->ngram_device != device) {
     cudaSetDevice(sc->ngram_device); cudaFree(sc->d_ngram); sc->d_ngram = nullptr; cudaSetDevice(device);
@@ -492,7 +493,12 @@ static int ensure_ngram_on_device(HostScorer *sc, int device) {
   std::vector<std::pair<const void *, size_t>> parts;
   parts.emplace_back(m.uni_prob.data(), m.uni_prob.size() * 4);
   parts.emplace_back(m.uni_backoff.data(), m.uni_backoff.size() * 4);
-  for (int n = 2; n <= m.order; ++n) parts.emplace_back(m.tables[n - 1].data(), m.tables[n - 1].size() * sizeof(NgramEntry));
+  for (int n = 2; n <= m.order; ++n) {
+    if (m.layout == kNgramKenlmProbing)  // a KenLM probing file's tables, byte for byte
+      parts.emplace_back(m.probing[n - 1].data(), m.probing[n - 1].size() * 8);
+    else
+      parts.emplace_back(m.tables[n - 1].data(), m.tables[n - 1].size() * sizeof(NgramEntry));
+  }
   parts.emplace_back(sc->word_of_state.data(), sc->word_of_state.size() * 4);
   parts.emplace_back(sc->label_word.data(), sc->label_word.size() * 4);
   parts.emplace_back(m.label_bytes.data(), m.label_bytes.size());
@@ -513,7 +519,10 @@ static int ensure_ngram_on_device(HostScorer *sc, int device) {
   size_t i = 0;
   v.uni_prob = reinterpret_cast<const float *>(d + off[i++]);
   v.uni_backoff = reinterpret_cast<const float *>(d + off[i++]);
-  for (int n = 2; n <= m.order; ++n) v.table[n - 1] = reinterpret_cast<const NgramEntry *>(d + off[i++]);
+  for (int n = 2; n <= m.order; ++n) {
+    if (m.layout == kNgramKenlmProbing) v.probe[n - 1] = reinterpret_cast<const uint32_t *>(d + off[i++]);
+    else v.table[n - 1] = reinterpret_cast<const NgramEntry *>(d + off[i++]);
+  }
   sc->d_word_of_state = reinterpret_cast<int *>(d + off[i++]);
   sc->d_label_word = reinterpret_cast<int *>(d + off[i++]);
   NgramFront f = m.front();
@@ -1443,7 +1452,7 @@ int ctcdec_scorer_create_arpa(const char *path, double alpha, double beta, const
     m->labels.emplace_back(labels[i] ? labels[i] : "");
     if (m->labels.back() == " ") m->space_id = i;  // reference Scorer::set_char_map (scorer.cpp:148-161)
   }
-  const std::string why = load_arpa(path, *m);
+  const std::string why = load_ngram_file(path, *m);
   if (!why.empty()) return fail(CTCDEC_E_UNSUPPORTED, "language model %s refused: %s", path, why.c_str());
   std::vector<const char *> words;
   for (const std::string &w : m->vocabulary) words.push_back(w.c_str());

@@ -25,7 +25,7 @@
 #include <vector>
 
 #include "../../include/ctcdecode_b200.h"
-#include "ngram_arpa.h"
+#include "ngram_kenlm.h"
 
 namespace ctc {
 

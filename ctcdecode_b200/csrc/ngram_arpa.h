@@ -1,8 +1,10 @@
-// Host side of the ARPA n-gram scorer: the loader that fills ngram_lm.h's tables, and the two scorer hooks
-// (ctcdec_scorer_hooks) computed from them exactly as the reference's Scorer computes them over KenLM.
+// Host side of the n-gram scorer: the model's tables (NgramModel), the ARPA text loader that fills them, and the two
+// scorer hooks (ctcdec_scorer_hooks) computed from them exactly as the reference's Scorer computes them over KenLM.
+// KenLM binary files are read by ngram_kenlm.h, whose load_ngram_file takes either form.
 //
-// The loader accepts only what it can reproduce exactly; everything else is refused with the reason:
-//   * a KenLM binary file, or anything that is not ARPA text ("\data\", counts, "\N-grams:" sections, "\end\");
+// The ARPA loader accepts only what it can reproduce exactly; everything else is refused with the reason:
+//   * a KenLM binary file (load_ngram_file sends those to ngram_kenlm.h), or anything that is not ARPA text ("\data\",
+//     counts, "\N-grams:" sections, "\end\");
 //   * order 1 (KenLM needs at least bigrams) or above kNgramMaxOrder;
 //   * counts that disagree with the sections, a malformed line, a duplicate n-gram or unigram;
 //   * an n-gram word that is not a unigram, a missing <s> or </s> (KenLM refuses all of these too);
@@ -29,6 +31,10 @@ struct NgramModel {
   std::unordered_map<std::string, int32_t> word_id;
   std::vector<float> uni_prob, uni_backoff;
   std::vector<NgramEntry> tables[kNgramMaxOrder];
+  // a KenLM probing file (layout kNgramKenlmProbing): its tables of orders 2..N byte for byte, instead of `tables`
+  int layout = kNgramTables;
+  std::vector<uint64_t> probing[kNgramMaxOrder];
+  uint32_t buckets[kNgramMaxOrder] = {};
   // the decoder's labels, for the label-id hooks (reference Scorer::set_char_map, scorer.cpp:148-161)
   std::vector<std::string> labels;
   int space_id = -1;  // the " " label, -1 if none (reference SPACE_ID_)
@@ -46,9 +52,15 @@ struct NgramModel {
     v.bos = id_of("<s>");
     v.uni_prob = uni_prob.data();
     v.uni_backoff = uni_backoff.data();
+    v.layout = layout;
     for (int n = 2; n <= order; ++n) {
-      v.table[n - 1] = tables[n - 1].data();
-      v.mask[n - 1] = (uint32_t)tables[n - 1].size() - 1;
+      if (layout == kNgramKenlmProbing) {
+        v.probe[n - 1] = reinterpret_cast<const uint32_t *>(probing[n - 1].data());
+        v.buckets[n - 1] = buckets[n - 1];
+      } else {
+        v.table[n - 1] = tables[n - 1].data();
+        v.mask[n - 1] = (uint32_t)tables[n - 1].size() - 1;
+      }
     }
     return v;
   }
@@ -104,6 +116,18 @@ static inline void ngram_build_front(NgramModel &m) {
     while (m.words[s].len >= 0) s = (s + 1) & mask;
     m.words[s] = e;
   }
+}
+
+// reference Scorer::load_lm (scorer.cpp:61-71): word-based as soon as one word other than <unk> / <s> / </s> is longer
+// than one UTF-8 character
+static inline int ngram_character_based(const std::vector<std::string> &vocabulary) {
+  for (const std::string &w : vocabulary) {
+    if (w == "<unk>" || w == "<s>" || w == "</s>") continue;
+    int chars = 0;
+    for (char c : w) chars += ((c & 0xc0) != 0x80);
+    if (chars > 1) return 0;
+  }
+  return 1;
 }
 
 namespace arpa_detail {
@@ -327,15 +351,7 @@ static inline std::string load_arpa(const char *path, NgramModel &m) {
 
   for (int n = 2; n <= order; ++n) ngram_build_table(entries[n - 1], n, m.tables[n - 1]);
 
-  // reference Scorer::load_lm (scorer.cpp:61-71): word-based as soon as one word other than <unk> / <s> / </s> is longer
-  // than one UTF-8 character
-  m.is_character_based = 1;
-  for (const std::string &w : m.vocabulary) {
-    if (w == "<unk>" || w == "<s>" || w == "</s>") continue;
-    int chars = 0;
-    for (char c : w) chars += ((c & 0xc0) != 0x80);
-    if (chars > 1) m.is_character_based = 0;
-  }
+  m.is_character_based = ngram_character_based(m.vocabulary);
   ngram_build_front(m);
   return "";
 }

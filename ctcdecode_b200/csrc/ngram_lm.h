@@ -1,18 +1,20 @@
-// N-gram language model read from an ARPA text file: the tables, the one lookup that reproduces the reference's
-// Scorer::get_log_cond_prob (scorer.cpp:74-93) over KenLM's probing model bit for bit, the reference's label-to-word
+// N-gram language model read from an ARPA text file or a KenLM binary file: the tables, the one lookup that reproduces
+// the reference's Scorer::get_log_cond_prob (scorer.cpp:74-93) over KenLM bit for bit, the reference's label-to-word
 // front end (make_ngram, split_labels, get_sent_log_prob) and the read-out rescoring of a result row.  All of it
-// compiles for the host and for the device (plain pointers: views of host vectors or of their HBM copies); the ARPA
-// loader and the building of the tables are host code (ngram_arpa.h).
+// compiles for the host and for the device (plain pointers: views of host vectors or of their HBM copies); the loaders
+// and the building of the tables are host code (ngram_arpa.h, ngram_kenlm.h).
 //
 // What is reproduced, from KenLM's query path (lm/model.cc FullScore / ResumeScore, lm/read_arpa.cc):
-//   * word ids: 0 is <unk> (also "<UNK>"), then the unigrams in file order; an unknown string is 0;
-//   * every stored log10 probability has its sign bit set (KenLM's Prob() does so; 0 becomes -0.0);
+//   * word ids: 0 is <unk> (also "<UNK>"), then the unigrams in file order (a binary file's own id order); an unknown
+//     string is 0;
+//   * log10 probabilities are read as KenLM returns them: from ARPA text and probing files with the sign bit set (its
+//     Prob() does so; 0 becomes -0.0), from a trie file as stored;
 //   * a backoff of 0 (or none) is stored as -0.0, "no n-gram extends this one", and turned into +0.0 when the n-gram is
 //     the context of a longer one: the sign decides how long the state's history is, as in KenLM;
 //   * a word is scored in the state left by the previous one: the longest matching n-gram's probability, then the
 //     state's context backoffs from the matched length up, added in float in that order.
-// The tables hold the file's n-grams plus the suffix entries KenLM fills in on load (ngram_arpa.h), so "not found"
-// means the same thing here as in KenLM.
+// The tables hold the file's n-grams plus the suffix entries KenLM fills in on load (ngram_arpa.h), or what a KenLM
+// binary file holds (ngram_kenlm.h), so "not found" means the same thing here as in KenLM.
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -36,15 +38,32 @@ struct NgramEntry {
   float prob, backoff;
 };
 
-// Read-only view of the tables: host vectors or their device copies.
+// How the tables of orders >= 2 are laid out.
+enum NgramLayout {
+  kNgramTables = 0,        // NgramEntry tables with the full key (ARPA text, KenLM tries unpacked on load)
+  kNgramKenlmProbing = 1,  // a KenLM probing file's own tables, searched by their 64-bit keys (ngram_probe)
+};
+
+// Read-only view of the tables: host vectors or their device copies.  It is a kernel parameter of the beam and read-out
+// kernels, and its size is kept: the two layouts share the per-order fields.
 struct NgramView {
   int order = 0;
   int vocab = 0;
   int bos = 0;                         // the id of "<s>"
-  const float *uni_prob = nullptr;     // [vocab]
+  int layout = kNgramTables;
+  const float *uni_prob = nullptr;     // [vocab]; a probing file's raw values, the sign bit its independent-left flag
   const float *uni_backoff = nullptr;  // [vocab]
-  const NgramEntry *table[kNgramMaxOrder] = {};  // [n - 1]: order n >= 2, capacity mask[n - 1] + 1 (a power of two)
-  uint32_t mask[kNgramMaxOrder] = {};
+  // [n - 1]: order n >= 2.  kNgramTables: capacity mask[n - 1] + 1 (a power of two).  kNgramKenlmProbing: the table's
+  // bytes, buckets[n - 1] entries of 16 bytes (key, prob, backoff) below the highest order and of 12 bytes (key, prob)
+  // at it, both packed to 4 bytes (so a key is read as two 32-bit words).
+  union {
+    const NgramEntry *table[kNgramMaxOrder] = {};
+    const uint32_t *probe[kNgramMaxOrder];
+  };
+  union {
+    uint32_t mask[kNgramMaxOrder] = {};
+    uint32_t buckets[kNgramMaxOrder];
+  };
 };
 
 struct NgramState {
@@ -81,25 +100,84 @@ CTC_NG_HD bool ngram_has_extension(float backoff) {
   return u != 0x80000000u;  // anything but -0.0
 }
 
-// KenLM GenericModel::FullScore(in, w, out).prob: log10 p(w | in's history).
+CTC_NG_HD uint32_t ngram_bits(float f) {
+  uint32_t u;
+  memcpy(&u, &f, 4);
+  return u;
+}
+CTC_NG_HD float ngram_float(uint32_t u) {
+  float f;
+  memcpy(&f, &u, 4);
+  return f;
+}
+
+// KenLM's key of an n-gram in a probing file (lm/search_hashed.hh CombineWordHash): it starts as the newest word's id,
+// and each older word is folded in.
+CTC_NG_HD uint64_t ngram_kenlm_combine(uint64_t key, int32_t older) {
+  return (key * 8978948897894561157ull) ^ ((uint64_t)(uint32_t)(1u + (uint32_t)older) * 17894857484156487943ull);
+}
+
+// The entry with this key in order n's probing table, or null: linear probing from key % buckets; key 0 is an empty
+// bucket (util/probing_hash_table.hh Find).
+CTC_NG_HD const uint32_t *ngram_probe(const NgramView &m, int n, uint64_t key) {
+  const uint32_t *t = m.probe[n - 1];
+  const uint32_t buckets = m.buckets[n - 1];
+  const uint32_t words = n < m.order ? 4 : 3;
+  for (uint64_t b = key % buckets;; b = b + 1 == buckets ? 0 : b + 1) {
+    const uint32_t *e = t + b * words;
+    const uint64_t got = (uint64_t)e[0] | ((uint64_t)e[1] << 32);
+    if (got == key) return e;
+    if (got == 0) return nullptr;
+  }
+}
+
+// The stored (prob, backoff) bits of the n-gram key[0..n) (text order) in either layout; false if it is not there.  A
+// probing file's key starts as the newest word's id and folds in the older words, newest first.
+CTC_NG_HD bool ngram_lookup(const NgramView &m, const int32_t *key, int n, uint32_t &prob, uint32_t &backoff) {
+  if (m.layout == kNgramKenlmProbing) {
+    uint64_t h = (uint32_t)key[n - 1];
+    for (int i = n - 2; i >= 0; --i) h = ngram_kenlm_combine(h, key[i]);
+    const uint32_t *e = ngram_probe(m, n, h);
+    if (!e) return false;
+    prob = e[2];
+    backoff = n < m.order ? e[3] : 0u;
+    return true;
+  }
+  const NgramEntry *e = ngram_find(m, key, n);
+  if (!e) return false;
+  prob = ngram_bits(e->prob);
+  backoff = ngram_bits(e->backoff);
+  return true;
+}
+
+// KenLM GenericModel::FullScore(in, w, out).prob: log10 p(w | in's history).  Only ngram_lookup depends on the layout.
+// A probing file's probabilities carry KenLM's independent-left flag in their sign bit: they are read as Prob() reads
+// them (sign set; the highest order's as stored), and a set flag ends the search, as in KenLM's ResumeScore.
 CTC_NG_HD float ngram_score(const NgramView &m, const NgramState &in, int32_t w, NgramState &out) {
+  const bool probing = m.layout == kNgramKenlmProbing;
   float prob = m.uni_prob[w];
+  bool stop = probing && (ngram_bits(prob) >> 31);
+  if (probing) prob = ngram_float(ngram_bits(prob) | 0x80000000u);
   out.backoff[0] = m.uni_backoff[w];
   out.len = ngram_has_extension(out.backoff[0]) ? 1 : 0;
   out.words[0] = w;
   int matched = 1;
   int32_t key[kNgramMaxOrder];
-  for (int j = 0; j < in.len; ++j) {  // the n-gram of the last j + 1 history words and w
+  for (int j = 0; j < in.len && !stop; ++j) {  // the n-gram of the last j + 1 history words and w
     const int n = j + 2;
     for (int i = 0; i <= j; ++i) key[i] = in.words[j - i];
     key[j + 1] = w;
-    const NgramEntry *e = ngram_find(m, key, n);
-    if (!e) break;
-    prob = e->prob;
+    uint32_t p, bo;
+    if (!ngram_lookup(m, key, n, p, bo)) break;
+    if (probing) {
+      stop = p >> 31;
+      if (n < m.order) p |= 0x80000000u;
+    }
+    prob = ngram_float(p);
     matched = n;
     if (n < m.order) {
-      out.backoff[j + 1] = e->backoff;
-      if (ngram_has_extension(e->backoff)) out.len = n;
+      out.backoff[j + 1] = ngram_float(bo);
+      if (ngram_has_extension(ngram_float(bo))) out.len = n;
     }
   }
   for (int i = 1; i < out.len; ++i) out.words[i] = in.words[i - 1];

@@ -16,7 +16,8 @@ Differences from the reference, all additive:
   * ``model_path`` (word-based KenLM models): the language model stays on the host behind a hook; the real Scorer
     comes from a provider library (``scorer_provider=`` / CTCDECODE_B200_SCORER_PROVIDER, see scorer.py and
     INTEGRATION.md; providers/ builds one from the reference's own Scorer + KenLM).  ``scorer_provider="device"``
-    needs no provider: the library reads an ARPA file itself and reproduces the reference Scorer bit for bit.  CUDA probabilities and logits
+    needs no provider: the library reads the ARPA or KenLM binary file itself (REST_PROBING binaries excepted) and
+    reproduces the reference Scorer bit for bit.  CUDA probabilities and logits
     stay on the GPU with a scorer too (ctcdec_decode_batch_lm_device); that call returns when the results are in place,
     because the host answers the beam kernel's per-frame LM handshake while it runs.  The online decoder takes a
     scorer too (device-resident states, one persistent launch per chunk).  Character-based models are detected like

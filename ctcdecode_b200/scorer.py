@@ -18,8 +18,10 @@ from the reference's sources where they lie: providers/_build/libkenlm_provider.
 provider is chosen with ``scorer_provider=`` or the environment variable CTCDECODE_B200_SCORER_PROVIDER.
 
 ``scorer_provider="device"`` (or CTCDECODE_B200_SCORER_PROVIDER=device) needs no provider: ``ArpaScorer`` has the
-library read an ARPA text file itself (ctcdec_scorer_create_arpa).  Its hooks reproduce the reference Scorer over
-KenLM bit for bit; a model they cannot reproduce exactly (a KenLM binary file, order above 6, ...) is refused.
+library read the model file itself (ctcdec_scorer_create_arpa): ARPA text, or a KenLM binary file of any type KenLM's
+build_binary writes but REST_PROBING (probing, trie, quantized and array-compressed tries).  Its hooks reproduce the
+reference Scorer over KenLM bit for bit; a model they cannot reproduce exactly (order above 6, REST_PROBING, a damaged
+binary, ...) is refused.
 """
 import ctypes
 import os
@@ -42,7 +44,8 @@ def make_scorer(labels, model_path, alpha, beta, provider=None):
 
 
 class ArpaScorer(object):
-    """The library-side scorer built from an ARPA file by the library itself (no provider library, no KenLM)."""
+    """The library-side scorer built from an ARPA or KenLM binary file by the library itself (no provider library, no
+    KenLM)."""
 
     def __init__(self, labels, model_path, alpha, beta):
         self.handle = None

@@ -170,7 +170,8 @@ typedef struct ctcdec_scorer_hooks {
 int ctcdec_scorer_create(const ctcdec_scorer_hooks *hooks, double alpha, double beta, const char *const *labels,
                          int n_labels, const char *const *words, int n_words, int max_order, int is_character_based,
                          void **scorer);
-/* The same scorer from an ARPA text file, with no hook to supply: the library reads the n-gram tables itself and its
+/* The same scorer from an ARPA text file or a KenLM binary file (told apart by the file's first bytes), with no hook to
+ * supply: the library reads the n-gram tables itself and its
  * own hooks reproduce the reference Scorer over KenLM (Scorer::get_log_cond_prob / get_sent_log_prob, scorer.cpp:74-120)
  * bit for bit: the longest matching n-gram, KenLM's float sum of context backoffs in KenLM's order, "<s>" padding scored
  * as words, any out-of-vocabulary word -1000.  Word-based or character-based is read from the vocabulary as
@@ -182,11 +183,19 @@ int ctcdec_scorer_create(const ctcdec_scorer_hooks *hooks, double alpha, double 
  * bytes (CTCDEC_E_UNSUPPORTED beyond 64 GiB).  The blocking entries rescore their results on the host, through this
  * scorer's hooks; ctcdec_decode_batch_lm_device_async and ctcdec_decode_stream_device rescore them on the device with
  * the same label-to-word front end over tables of the labels' bytes and the unigrams' spellings.
+ * KenLM binary files (format version 5, as build_binary writes them): PROBING files keep their own hash tables, which
+ * go to the device byte for byte and are searched there as KenLM searches them; TRIE, QUANT_TRIE, ARRAY_TRIE and
+ * QUANT_ARRAY_TRIE files are unpacked on load into the ARPA tables, with the values KenLM reads from the file
+ * (dequantized with the file's own bins), at 32 bytes per n-gram in device memory.  The word ids are the file's.
  * Refused with CTCDEC_E_UNSUPPORTED, the reason in ctcdec_last_error(), anything the tables cannot reproduce exactly:
- * a KenLM binary file or other non-ARPA input, order 1 or above 6, counts that disagree with the sections, a malformed
- * line, a duplicate entry, an n-gram word missing from the unigrams, no <s> or </s>, an n-gram whose context or suffix
- * n-gram is missing (KenLM would fill it in on load), a positive log-prob, a NaN or +inf log-prob, a non-finite
- * backoff.  A file that cannot be opened is CTCDEC_E_INVALID. */
+ * ARPA text: non-ARPA input, order 1 or above 6, counts that disagree with the sections, a malformed line, a duplicate
+ * entry, an n-gram word missing from the unigrams, no <s> or </s>, an n-gram whose context is missing, a positive
+ * log-prob, a NaN or +inf log-prob, a non-finite backoff.  A binary file (the reason says "KenLM binary"): a truncated
+ * file or header, an unfinished build, a version other than 5, other endianness or type sizes, REST_PROBING, an
+ * unknown model type or search version, order 1 or above 6, no vocabulary strings or a word count that disagrees
+ * with the header, no <s> or </s>, region sizes that disagree with the file's length, a probing table with no empty
+ * bucket, trie word ids or pointers out of range or out of order.  A file that cannot be opened is
+ * CTCDEC_E_INVALID. */
 int ctcdec_scorer_create_arpa(const char *path, double alpha, double beta, const char *const *labels, int n_labels,
                               void **scorer);
 /* Diagnostic: the scorer's hooks on one label-id prefix -- cond_log_prob and sent_log_prob of ctcdec_scorer_hooks, for a

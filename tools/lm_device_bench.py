@@ -6,7 +6,7 @@ beta 1.0) through CTCBeamDecoder three ways:
   device          CUDA probabilities through the device entry point (ctcdec_decode_batch_lm_device)
   logits_f16      decode_logits of fp16 logits (the device entry, the log-softmax taken by the scan kernel)
 
-    python tools/lm_device_bench.py [--reps N] [--device I] [--scorer hook|device|async]
+    python tools/lm_device_bench.py [--reps N] [--device I] [--scorer hook|device|async] [--model PATH]
 
 --scorer device times the library's own ARPA scorer (scorer_provider="device": the beam kernel computes the LM terms,
 no per-frame host handshake) against the hook scorer on the same CUDA probabilities instead:
@@ -22,6 +22,9 @@ no per-frame host handshake) against the hook scorer on the same CUDA probabilit
   graph           the async decode captured once into a CUDA graph, replayed
 
 and, in a separate profiled pass afterwards, the CUDA time of the read-out kernel alone (torch.profiler).
+
+--model decodes with another language model than test.arpa, for instance a KenLM binary file written from it by
+build_binary (probing or trie): the device scorer and the hook scorer both read it.
 
 Every path is warmed up, then timed N times in alternating rounds with a host clock around the call and a device
 synchronise after it.  Prints one JSON line: per path the median and the spread of the call time
@@ -69,6 +72,7 @@ def main():
     ap.add_argument("--scorer", choices=["hook", "device", "async"], default="hook",
                     help="hook: the three input paths of the hook scorer; device: the device scorer against the hook; "
                          "async: the device scorer's blocking, asynchronous and graph-replayed decodes")
+    ap.add_argument("--model", default=TINY_LM, help="the language model (ARPA text or a KenLM binary file)")
     args = ap.parse_args()
     dev = torch.device("cuda", args.device)
     torch.cuda.set_device(dev)
@@ -77,7 +81,7 @@ def main():
     probs = c5_inputs(B, T, 0)
     probs_d = probs.to(dev)
     logits = probs_d.clamp_min(1e-20).log().mul(1.25).half()
-    kw = dict(model_path=TINY_LM, alpha=cfg["alpha"], beta=cfg["beta"], beam_width=cfg["beam"],
+    kw = dict(model_path=args.model, alpha=cfg["alpha"], beta=cfg["beta"], beam_width=cfg["beam"],
               cutoff_top_n=cfg["cutoff_top_n"], cutoff_prob=cfg["cutoff_prob"])
     readout_ms = None
     if args.scorer == "async":
@@ -142,7 +146,8 @@ def main():
         ks = [e.device_time for e in prof.events() if "lm_readout_kernel" in e.name]
         readout_ms = {"ms_median": statistics.median(ks) / 1e3, "ms_min": min(ks) / 1e3, "ms_max": max(ks) / 1e3,
                       "launches": len(ks)} if ks else None
-    print(json.dumps({"workload": cfg["name"], "scorer": args.scorer, "card": card_info(args.device), "paths": legs,
+    print(json.dumps({"workload": cfg["name"], "scorer": args.scorer, "model": os.path.basename(args.model),
+                      "library": os.environ.get("CTCDECODE_B200_LIB") or "in-tree", "card": card_info(args.device), "paths": legs,
                       "readout_kernel": readout_ms,
                       ("all_arms_identical" if args.scorer == "async" else "%s_%s_identical" % compared): bool(same),
                       "note": "host clock around each call and a device synchronise after it; paths alternate within "
