@@ -53,6 +53,7 @@ _SIGNATURES = {
     "ctcdec_scorer_is_character_based": (ctypes.c_int, [_vp]),
     "ctcdec_scorer_max_order": (ctypes.c_int, [_vp]),
     "ctcdec_scorer_dict_size": (ctypes.c_int, [_vp]),
+    "ctcdec_scorer_table_bytes": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_size_t)]),
     "ctcdec_scorer_reset_params": (ctypes.c_int, [_vp, ctypes.c_double, ctypes.c_double]),
     "ctcdec_decode_batch_lm_host": (ctypes.c_int, [ctypes.POINTER(Config), _vp, _vp, _vp, ctypes.c_int, ctypes.c_int,
                                                    _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int]),

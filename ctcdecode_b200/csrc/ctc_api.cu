@@ -493,11 +493,16 @@ static int ensure_ngram_on_device(HostScorer *sc, int device) {
   std::vector<std::pair<const void *, size_t>> parts;
   parts.emplace_back(m.uni_prob.data(), m.uni_prob.size() * 4);
   parts.emplace_back(m.uni_backoff.data(), m.uni_backoff.size() * 4);
-  for (int n = 2; n <= m.order; ++n) {
-    if (m.layout == kNgramKenlmProbing)  // a KenLM probing file's tables, byte for byte
-      parts.emplace_back(m.probing[n - 1].data(), m.probing[n - 1].size() * 8);
-    else
-      parts.emplace_back(m.tables[n - 1].data(), m.tables[n - 1].size() * sizeof(NgramEntry));
+  if (m.layout == kNgramKenlmTrie) {  // a KenLM trie file's search region, byte for byte, and its order descriptors
+    parts.emplace_back(m.trie_bits.data(), m.trie_bits.size() * 8);
+    parts.emplace_back(m.trie_orders.data(), m.trie_orders.size() * sizeof(NgramTrieOrder));
+  } else {
+    for (int n = 2; n <= m.order; ++n) {
+      if (m.layout == kNgramKenlmProbing)  // a KenLM probing file's tables, byte for byte
+        parts.emplace_back(m.probing[n - 1].data(), m.probing[n - 1].size() * 8);
+      else
+        parts.emplace_back(m.tables[n - 1].data(), m.tables[n - 1].size() * sizeof(NgramEntry));
+    }
   }
   parts.emplace_back(sc->word_of_state.data(), sc->word_of_state.size() * 4);
   parts.emplace_back(sc->label_word.data(), sc->label_word.size() * 4);
@@ -519,9 +524,14 @@ static int ensure_ngram_on_device(HostScorer *sc, int device) {
   size_t i = 0;
   v.uni_prob = reinterpret_cast<const float *>(d + off[i++]);
   v.uni_backoff = reinterpret_cast<const float *>(d + off[i++]);
-  for (int n = 2; n <= m.order; ++n) {
-    if (m.layout == kNgramKenlmProbing) v.probe[n - 1] = reinterpret_cast<const uint32_t *>(d + off[i++]);
-    else v.table[n - 1] = reinterpret_cast<const NgramEntry *>(d + off[i++]);
+  if (m.layout == kNgramKenlmTrie) {
+    v.trie.bits = reinterpret_cast<const uint64_t *>(d + off[i++]);
+    v.trie.orders = reinterpret_cast<const NgramTrieOrder *>(d + off[i++]);
+  } else {
+    for (int n = 2; n <= m.order; ++n) {
+      if (m.layout == kNgramKenlmProbing) v.probe[n - 1] = reinterpret_cast<const uint32_t *>(d + off[i++]);
+      else v.table[n - 1] = reinterpret_cast<const NgramEntry *>(d + off[i++]);
+    }
   }
   sc->d_word_of_state = reinterpret_cast<int *>(d + off[i++]);
   sc->d_label_word = reinterpret_cast<int *>(d + off[i++]);
@@ -1463,6 +1473,14 @@ int ctcdec_scorer_create_arpa(const char *path, double alpha, double beta, const
   HostScorer *sc = static_cast<HostScorer *>(*scorer);
   sc->ngram = m;
   lm_dev_word_ids(*sc);
+  return CTCDEC_OK;
+}
+
+int ctcdec_scorer_table_bytes(const void *scorer, size_t *bytes) {
+  if (!scorer || !bytes) return fail(CTCDEC_E_INVALID, "bad scorer / bytes argument");
+  const HostScorer *sc = static_cast<const HostScorer *>(scorer);
+  if (!sc->ngram) return fail(CTCDEC_E_UNSUPPORTED, "table_bytes takes a scorer from ctcdec_scorer_create_arpa only");
+  *bytes = sc->ngram->table_bytes();
   return CTCDEC_OK;
 }
 

@@ -35,6 +35,9 @@ struct NgramModel {
   int layout = kNgramTables;
   std::vector<uint64_t> probing[kNgramMaxOrder];
   uint32_t buckets[kNgramMaxOrder] = {};
+  // a KenLM trie file (layout kNgramKenlmTrie): its search region byte for byte, zero-padded, and where each order is
+  std::vector<uint64_t> trie_bits;
+  std::vector<NgramTrieOrder> trie_orders;
   // the decoder's labels, for the label-id hooks (reference Scorer::set_char_map, scorer.cpp:148-161)
   std::vector<std::string> labels;
   int space_id = -1;  // the " " label, -1 if none (reference SPACE_ID_)
@@ -53,6 +56,11 @@ struct NgramModel {
     v.uni_prob = uni_prob.data();
     v.uni_backoff = uni_backoff.data();
     v.layout = layout;
+    if (layout == kNgramKenlmTrie) {
+      v.trie.bits = trie_bits.data();
+      v.trie.orders = trie_orders.data();
+      return v;
+    }
     for (int n = 2; n <= order; ++n) {
       if (layout == kNgramKenlmProbing) {
         v.probe[n - 1] = reinterpret_cast<const uint32_t *>(probing[n - 1].data());
@@ -80,6 +88,13 @@ struct NgramModel {
   int32_t id_of(const std::string &w) const {
     auto it = word_id.find(w);
     return it == word_id.end() ? 0 : it->second;
+  }
+  // The bytes of n-gram data a device holds: the unigrams and the data of orders >= 2 (the trie's order descriptors,
+  // a few hundred bytes, aside).
+  size_t table_bytes() const {
+    size_t bytes = (uni_prob.size() + uni_backoff.size()) * 4 + trie_bits.size() * 8;
+    for (int n = 2; n <= order; ++n) bytes += tables[n - 1].size() * sizeof(NgramEntry) + probing[n - 1].size() * 8;
+    return bytes;
   }
 };
 

@@ -9,10 +9,11 @@
 //   * PROBING (type 0): the unigram array is split into uni_prob / uni_backoff, and the tables of orders 2..N are kept
 //     byte for byte (NgramModel::probing) and searched as they are (ngram_lm.h ngram_probe): their keys are 64-bit
 //     hashes of word ids, from which the n-grams cannot be recovered;
-//   * TRIE, QUANT_TRIE, ARRAY_TRIE, QUANT_ARRAY_TRIE (types 2-5): the reversed trie is walked once and every n-gram it
-//     holds is stored in text order with the values KenLM's FullScore reads for it (bit-packed word ids and pointers,
-//     Bhiksha-compressed pointers, the file's own quantization bins), in the full-key tables of ngram_arpa.h.  The file
-//     already holds the entries build_binary filled in for pruned suffixes, so nothing is added.
+//   * TRIE, QUANT_TRIE, ARRAY_TRIE, QUANT_ARRAY_TRIE (types 2-5): the search region (quantization bins, unigram
+//     records, Bhiksha offset arrays, bit-packed orders) is kept byte for byte (NgramModel::trie_bits) with a
+//     descriptor per order, and searched as it is (ngram_lm.h ngram_trie_step), after one validation pass
+//     (trie_validate) that makes every search end inside the region.  The file already holds the entries build_binary
+//     filled in for pruned suffixes, so nothing is added.
 // Refused, with the reason (all before anything reaches the device): a truncated file or header, the "incomplete" magic,
 // a version other than 5, other test values, REST_PROBING (type 1, build_binary -r), an unknown model type or search
 // version, order 1 or above kNgramMaxOrder, no vocabulary strings or a word count that disagrees with the header, no
@@ -66,15 +67,7 @@ struct File {
     memcpy(&v, b.data() + off, sizeof(T));
     return v;
   }
-  uint64_t bits64(uint64_t base, uint64_t bit) const { return at<uint64_t>(base + (bit >> 3)) >> (bit & 7); }
-  uint32_t bits32(uint64_t base, uint64_t bit) const { return at<uint32_t>(base + (bit >> 3)) >> (bit & 7); }
 };
-
-inline float as_float(uint32_t u) {
-  float f;
-  memcpy(&f, &u, 4);
-  return f;
-}
 
 // Pointer compression of the array tries (lm/bhiksha.cc): how many high bits of a next pointer move to the offset array.
 inline uint8_t chop_bits(uint64_t max_offset, uint64_t max_next, uint8_t configured) {
@@ -95,10 +88,6 @@ struct PackedOrder {
   uint8_t word_bits = 0, quant_bits = 0, inline_bits = 0, total_bits = 0;
   // array tries: the offset array (file offset, count) whose index gives a next pointer's high bits
   uint64_t offsets = 0, n_offsets = 0;
-  uint64_t word(const File &f, uint64_t i) const {
-    return f.bits64(base, i * total_bits) & ((1ull << word_bits) - 1);
-  }
-  uint64_t value_bit(uint64_t i) const { return i * total_bits + word_bits; }
 };
 
 // TrieSearch::Size's pieces for one middle order (trie.cc BitPackedMiddle::Size, bhiksha.cc).
@@ -137,6 +126,69 @@ inline uint64_t longest_size(uint8_t quant_bits, uint64_t entries, uint64_t max_
     o->total_bits = total;
   }
   return ((1 + entries) * total + 7) / 8 + 8;
+}
+
+// The pointers of order q over [i, ...) read in increasing index order (the unigram records' `next` for q == 1).  An
+// array trie's high bits come from a walk along the offset array; with its first value 0 and its values in order that
+// is the same index the search's binary search (ngram_trie_next) finds.
+struct PointerWalk {
+  const uint64_t *b;
+  const NgramTrieOrder &o;
+  bool unigrams;
+  uint64_t k = 0;
+  uint64_t at(uint64_t i) {
+    if (unigrams) return ngram_trie_read(b, o.bit + 128 * i + 64);
+    uint64_t v = ngram_trie_field(b, o.bit + i * o.total_bits + o.word_bits + o.quant_bits, o.inline_bits);
+    if (o.n_offsets) {
+      while (k + 1 < o.n_offsets && ngram_trie_read(b, o.offsets + 64 * (k + 1)) <= i) ++k;
+      v |= k << o.inline_bits;
+    }
+    return v;
+  }
+};
+
+// One pass over the trie from the unigrams down, through the nodes a search can reach: every node's child range lies
+// within the next order's array and ranges follow each other (pointers never decrease), and the word ids of a node are
+// in the vocabulary and increasing.  A search in a trie that passes stays in bounds and finds what a full-key table
+// would.  Reads the region sequentially and allocates nothing.  Returns "" or the reason.
+inline std::string trie_validate(const NgramModel &m, uint64_t bound) {
+  const uint64_t *b = m.trie_bits.data();
+  const int order = m.order;
+  uint64_t lo = 0, hi = bound;  // the parents (order n - 1) reachable from the unigrams
+  for (int n = 2; n <= order; ++n) {
+    const NgramTrieOrder &parent = m.trie_orders[n - 2], &o = m.trie_orders[n - 1];
+    uint64_t c_lo, c_hi;
+    {
+      PointerWalk walk{b, parent, n == 2};
+      c_lo = c_hi = walk.at(lo);
+      for (uint64_t p = lo + 1; p <= hi; ++p) {
+        const uint64_t v = walk.at(p);
+        if (v < c_hi) return "a trie pointer of order " + std::to_string(n - 1) + " decreases";
+        c_hi = v;
+      }
+      if (c_hi > o.entries) return "a trie pointer of order " + std::to_string(n - 1) + " points past its array";
+    }
+    if (o.offsets) {
+      if (o.n_offsets == 0 || ngram_trie_read(b, o.offsets) != 0) return "array-compressed pointers do not start at 0";
+      for (uint64_t j = 1; j < o.n_offsets; ++j)
+        if (ngram_trie_read(b, o.offsets + 64 * j) < ngram_trie_read(b, o.offsets + 64 * (j - 1)))
+          return "array-compressed pointers out of order";
+    }
+    PointerWalk walk{b, parent, n == 2};
+    uint64_t c = walk.at(lo);
+    for (uint64_t p = lo; p < hi; ++p) {
+      const uint64_t end = walk.at(p + 1);
+      for (uint64_t first = c, prev_word = 0; c < end; ++c) {
+        const uint64_t w = ngram_trie_field(b, o.bit + c * o.total_bits, o.word_bits);
+        if (w >= bound) return "a trie word id of order " + std::to_string(n) + " is outside the vocabulary";
+        if (c > first && w <= prev_word) return "trie words of order " + std::to_string(n) + " out of order";
+        prev_word = w;
+      }
+    }
+    lo = c_lo;
+    hi = c_hi;
+  }
+  return "";
 }
 
 }  // namespace kenlm_detail
@@ -243,6 +295,9 @@ static inline std::string load_kenlm_binary(const char *path, NgramModel &m) {
       if (f.at<uint8_t>(at) != 0) return kb + "pointer compression version " + std::to_string(f.at<uint8_t>(at));
       bhiksha_bits = f.at<uint8_t>(at + 1);
     }
+    for (int n = 2; n <= order; ++n)  // (the search keeps entry indices in 32 bits)
+      if (counts[n - 1] >= (1ull << 32))
+        return kb + "the " + std::to_string(n) + "-gram trie array has 2^32 entries or more";
     const uint8_t middle_bits = quant ? (uint8_t)(prob_bits + backoff_bits) : 63;
     for (int n = 2; n < order; ++n)
       at += middle_size(array, bhiksha_bits, middle_bits, counts[n - 1], counts[0], counts[n], &packed[n - 1], at);
@@ -298,88 +353,43 @@ static inline std::string load_kenlm_binary(const char *path, NgramModel &m) {
       m.buckets[n - 1] = (uint32_t)buckets[n - 1];
     }
   } else {
-    m.layout = kNgramTables;
-    const uint64_t bins = search_at + 8;  // quantized tries: [order - 2] x (prob bins, backoff bins), then the longest's
-    const uint64_t per_order = ((1ull << prob_bits) + (1ull << backoff_bits)) * 4;
-    auto prob_bin = [&](int n, uint64_t code) { return f.at<float>(bins + (n - 2) * per_order + 4 * code); };
-    auto backoff_bin = [&](int n, uint64_t code) {
-      return f.at<float>(bins + (n - 2) * per_order + (1ull << prob_bits) * 4 + 4 * code);
-    };
+    // the search region, byte for byte: quantization header and bins, unigram records, and per order the offset array
+    // (array tries) and the bit-packed entries
+    m.layout = kNgramKenlmTrie;
+    const uint64_t region = at - search_at;
+    m.trie_bits.assign((region + 7) / 8 + 1, 0);
+    memcpy(m.trie_bits.data(), f.b.data() + search_at, region);
+    m.trie_orders.assign(order, NgramTrieOrder());
+    m.trie_orders[0].bit = (uni_at - search_at) * 8;
+    m.trie_orders[0].entries = bound;
     m.uni_prob.resize(bound);
     m.uni_backoff.resize(bound);
-    std::vector<uint64_t> next(bound + 1);  // the parents' next pointers, over the parents' index range [lo, hi]
-    for (uint64_t i = 0; i <= bound; ++i) {
-      if (i < bound) {
-        m.uni_prob[i] = f.at<float>(uni_at + 16 * i);
-        m.uni_backoff[i] = f.at<float>(uni_at + 16 * i + 4);
-      }
-      next[i] = f.at<uint64_t>(uni_at + 16 * i + 8);
+    for (uint64_t i = 0; i < bound; ++i) {
+      m.uni_prob[i] = f.at<float>(uni_at + 16 * i);
+      m.uni_backoff[i] = f.at<float>(uni_at + 16 * i + 4);
     }
-    std::vector<NgramEntry> parents;  // order n - 1's entries, indexed from lo (the unigrams: none, the id is the index)
-    uint64_t lo = 0;
+    const uint64_t per_order = ((1ull << prob_bits) + (1ull << backoff_bits)) * 4;
     for (int n = 2; n <= order; ++n) {
-      const PackedOrder &o = packed[n - 1];
-      const uint64_t hi = lo + next.size() - 1;
-      for (size_t k = 1; k < next.size(); ++k)
-        if (next[k] < next[k - 1]) return kb + "a trie pointer of order " + std::to_string(n - 1) + " decreases";
-      if (next.back() > o.entries)
-        return kb + "a trie pointer of order " + std::to_string(n - 1) + " points past its array";
-      const uint64_t c_lo = next.front(), c_hi = next.back();
-      std::vector<uint64_t> child_next;
-      if (n < order) {  // next pointers of the children c_lo .. c_hi (inclusive: the last one's end)
-        child_next.resize(c_hi - c_lo + 1);
-        uint64_t k = 0;  // array tries: the last offset-array index whose value is <= the entry's index
-        for (uint64_t c = c_lo; c <= c_hi; ++c) {
-          uint64_t v = f.bits64(o.base, o.value_bit(c) + o.quant_bits) & ((1ull << o.inline_bits) - 1);
-          if (array) {
-            if (c == c_lo) {
-              if (o.n_offsets == 0 || f.at<uint64_t>(o.offsets) != 0)
-                return kb + "array-compressed pointers do not start at 0";
-              for (uint64_t j = 1; j < o.n_offsets; ++j)
-                if (f.at<uint64_t>(o.offsets + 8 * j) < f.at<uint64_t>(o.offsets + 8 * (j - 1)))
-                  return kb + "array-compressed pointers out of order";
-            }
-            while (k + 1 < o.n_offsets && f.at<uint64_t>(o.offsets + 8 * (k + 1)) <= c) ++k;
-            v |= k << o.inline_bits;
-          }
-          child_next[c - c_lo] = v;
-        }
+      const PackedOrder &p = packed[n - 1];
+      NgramTrieOrder &o = m.trie_orders[n - 1];
+      o.bit = (p.base - search_at) * 8;
+      o.entries = p.entries;
+      o.word_bits = p.word_bits;
+      o.quant_bits = p.quant_bits;
+      o.inline_bits = p.inline_bits;
+      o.total_bits = p.total_bits;
+      if (array && n < order) {
+        o.offsets = (p.offsets - search_at) * 8;
+        o.n_offsets = p.n_offsets;
       }
-      std::vector<NgramEntry> children(c_hi - c_lo);
-      for (uint64_t p = lo; p < hi; ++p) {
-        uint64_t prev_word = 0;
-        for (uint64_t c = next[p - lo]; c < next[p - lo + 1]; ++c) {
-          const uint64_t w = o.word(f, c);
-          if (w >= bound) return kb + "a trie word id of order " + std::to_string(n) + " is outside the vocabulary";
-          if (c > next[p - lo] && w <= prev_word)
-            return kb + "trie words of order " + std::to_string(n) + " out of order";
-          prev_word = w;
-          NgramEntry &e = children[c - c_lo];
-          for (int k = 0; k < kNgramMaxOrder; ++k) e.w[k] = -1;
-          e.w[0] = (int32_t)w;  // the new word extends the parent's n-gram to the left
-          if (n == 2) e.w[1] = (int32_t)p;
-          else for (int k = 0; k < n - 1; ++k) e.w[k + 1] = parents[p - lo].w[k];
-          const uint64_t vb = o.value_bit(c);
-          if (n < order) {
-            if (quant) {
-              e.backoff = backoff_bin(n, f.bits32(o.base, vb) & ((1u << backoff_bits) - 1));
-              e.prob = prob_bin(n, f.bits32(o.base, vb + backoff_bits) & ((1u << prob_bits) - 1));
-            } else {
-              e.prob = as_float((uint32_t)f.bits64(o.base, vb) | 0x80000000u);
-              e.backoff = as_float((uint32_t)f.bits64(o.base, vb + 31));
-            }
-          } else {
-            e.prob = quant ? prob_bin(n, f.bits32(o.base, vb) & ((1u << prob_bits) - 1))
-                           : as_float((uint32_t)f.bits64(o.base, vb) | 0x80000000u);
-            e.backoff = -0.0f;
-          }
-        }
+      if (quant) {  // the bins after the 8-byte quantization header: per middle order prob then backoff, then the longest's
+        o.prob_bits = prob_bits;
+        o.backoff_bits = backoff_bits;
+        o.prob_bins = (8 + (n - 2) * per_order) * 8;
+        o.backoff_bins = o.prob_bins + (1ull << prob_bits) * 32;
       }
-      ngram_build_table(children, n, m.tables[n - 1]);
-      parents.swap(children);
-      next.swap(child_next);
-      lo = c_lo;
     }
+    if (const std::string why = trie_validate(m, bound); !why.empty()) return kb + why;
   }
   m.is_character_based = ngram_character_based(m.vocabulary);
   ngram_build_front(m);

@@ -40,12 +40,34 @@ struct NgramEntry {
 
 // How the tables of orders >= 2 are laid out.
 enum NgramLayout {
-  kNgramTables = 0,        // NgramEntry tables with the full key (ARPA text, KenLM tries unpacked on load)
+  kNgramTables = 0,        // NgramEntry tables with the full key (ARPA text)
   kNgramKenlmProbing = 1,  // a KenLM probing file's own tables, searched by their 64-bit keys (ngram_probe)
+  kNgramKenlmTrie = 2,     // a KenLM trie file's search data, walked as it is (ngram_trie_*)
+};
+
+// Where one order's data lies in a KenLM trie file's search region (NgramTrie::bits); all positions are in bits from
+// the region's start.  Order n >= 2 (index n - 1): entry i has its word id at bit + i * total_bits, then quant_bits of
+// value (unquantized: a 31-bit probability without its sign, then a 32-bit backoff below the highest order; quantized:
+// the backoff code, then the probability code), then, below the highest order, the low inline_bits of its next
+// pointer.  Index 0 describes the unigram array of {float prob, float backoff, uint64 next} records.
+struct NgramTrieOrder {
+  uint64_t bit = 0;          // entry 0 (n >= 2), or the unigram array (index 0)
+  uint64_t entries = 0;      // entries of the order (the array has one more, the last pointer's end)
+  uint64_t offsets = 0;      // array tries, n < order: the offset array of n_offsets uint64 values (lm/bhiksha.cc);
+  uint64_t n_offsets = 0;    // a next pointer's high bits are the last index whose value is <= the entry's index
+  uint64_t prob_bins = 0, backoff_bins = 0;  // quantized: this order's bins, 2^prob_bits / 2^backoff_bits floats
+  uint8_t word_bits = 0, quant_bits = 0, inline_bits = 0, total_bits = 0;
+  uint8_t prob_bits = 0, backoff_bits = 0;   // 0: unquantized
+};
+
+// A trie file's search region (8-byte aligned, zero-padded by at least 8 bytes) and its order descriptors [order].
+struct NgramTrie {
+  const uint64_t *bits;
+  const NgramTrieOrder *orders;
 };
 
 // Read-only view of the tables: host vectors or their device copies.  It is a kernel parameter of the beam and read-out
-// kernels, and its size is kept: the two layouts share the per-order fields.
+// kernels, and its size is kept: the layouts share the per-order fields.
 struct NgramView {
   int order = 0;
   int vocab = 0;
@@ -55,10 +77,11 @@ struct NgramView {
   const float *uni_backoff = nullptr;  // [vocab]
   // [n - 1]: order n >= 2.  kNgramTables: capacity mask[n - 1] + 1 (a power of two).  kNgramKenlmProbing: the table's
   // bytes, buckets[n - 1] entries of 16 bytes (key, prob, backoff) below the highest order and of 12 bytes (key, prob)
-  // at it, both packed to 4 bytes (so a key is read as two 32-bit words).
+  // at it, both packed to 4 bytes (so a key is read as two 32-bit words).  kNgramKenlmTrie: `trie`, for all orders.
   union {
     const NgramEntry *table[kNgramMaxOrder] = {};
     const uint32_t *probe[kNgramMaxOrder];
+    NgramTrie trie;
   };
   union {
     uint32_t mask[kNgramMaxOrder] = {};
@@ -150,11 +173,79 @@ CTC_NG_HD bool ngram_lookup(const NgramView &m, const int32_t *key, int n, uint3
   return true;
 }
 
-// KenLM GenericModel::FullScore(in, w, out).prob: log10 p(w | in's history).  Only ngram_lookup depends on the layout.
+// ---- a KenLM trie file searched where it is (lm/search_trie.hh TrieSearch, lm/trie.cc, lm/bhiksha.cc) ----
+
+// The 64 bits of the trie region from bit `bit` on.  Two aligned 64-bit loads and a shift: the packed fields start at
+// any bit and straddle words, and an unaligned 8-byte load is a fault on the device.  The region's zero padding keeps
+// the second word inside it.
+CTC_NG_HD uint64_t ngram_trie_read(const uint64_t *b, uint64_t bit) {
+  const uint64_t i = bit >> 6;
+  const unsigned s = (unsigned)(bit & 63);
+  const uint64_t lo = b[i];
+  return s ? (lo >> s) | (b[i + 1] << (64 - s)) : lo;
+}
+
+CTC_NG_HD uint64_t ngram_trie_field(const uint64_t *b, uint64_t bit, unsigned width) {
+  return ngram_trie_read(b, bit) & ((1ull << width) - 1);
+}
+
+// The next pointer of entry i of order n < order: the start of its children's range in order n + 1.
+CTC_NG_HD uint64_t ngram_trie_next(const uint64_t *b, const NgramTrieOrder &o, uint64_t i) {
+  uint64_t v = ngram_trie_field(b, o.bit + i * o.total_bits + o.word_bits + o.quant_bits, o.inline_bits);
+  if (o.n_offsets) {  // array trie: the last offset index whose value is <= i (the first is 0, so there is one)
+    uint64_t lo = 1, hi = o.n_offsets;
+    while (lo < hi) {
+      const uint64_t mid = lo + (hi - lo) / 2;
+      if (ngram_trie_read(b, o.offsets + 64 * mid) <= i) lo = mid + 1;
+      else hi = mid;
+    }
+    v |= (lo - 1) << o.inline_bits;
+  }
+  return v;
+}
+
+// Searches order n's entries [lo, hi) (one node's children: word ids unique and increasing) for `word`.  On a match
+// the (prob, backoff) bits KenLM's FullScore reads for the entry, and, below the highest order, [lo, hi) becomes the
+// entry's children's range.  Entry indices fit 32 bits (the loader refuses larger orders): 64-bit ranges would make the
+// read-out kernel spill.
+CTC_NG_HD bool ngram_trie_step(const NgramView &m, int n, int32_t word, uint32_t &lo, uint32_t &hi, uint32_t &prob,
+                               uint32_t &backoff) {
+  const uint64_t *b = m.trie.bits;
+  const NgramTrieOrder &o = m.trie.orders[n - 1];
+  const uint64_t total = o.total_bits;
+  uint32_t a = lo, z = hi, i = 0;
+  bool found = false;
+  while (a < z && !found) {
+    i = a + (z - a) / 2;
+    const uint64_t got = ngram_trie_field(b, o.bit + i * total, o.word_bits);
+    found = got == (uint64_t)(uint32_t)word;
+    if (got < (uint64_t)(uint32_t)word) a = i + 1;
+    else z = i;
+  }
+  if (!found) return false;
+  const uint64_t vb = o.bit + i * total + o.word_bits;
+  if (o.prob_bits) {  // quantized: the backoff code first (below the highest order), then the probability code
+    const unsigned bb = n < m.order ? o.backoff_bits : 0;
+    prob = (uint32_t)ngram_trie_read(b, o.prob_bins + 32 * ngram_trie_field(b, vb + bb, o.prob_bits));
+    backoff = bb ? (uint32_t)ngram_trie_read(b, o.backoff_bins + 32 * ngram_trie_field(b, vb, bb)) : 0x80000000u;
+  } else {  // the sign bit is not stored; the backoff follows the probability's 31 bits
+    prob = (uint32_t)ngram_trie_read(b, vb) | 0x80000000u;
+    backoff = n < m.order ? (uint32_t)ngram_trie_read(b, vb + 31) : 0x80000000u;
+  }
+  if (n < m.order) {
+    lo = (uint32_t)ngram_trie_next(b, o, i);
+    hi = (uint32_t)ngram_trie_next(b, o, i + 1);
+  }
+  return true;
+}
+
+// KenLM GenericModel::FullScore(in, w, out).prob: log10 p(w | in's history).  Only the search depends on the layout.
 // A probing file's probabilities carry KenLM's independent-left flag in their sign bit: they are read as Prob() reads
-// them (sign set; the highest order's as stored), and a set flag ends the search, as in KenLM's ResumeScore.
+// them (sign set; the highest order's as stored), and a set flag ends the search, as in KenLM's ResumeScore.  A trie
+// is walked from w's unigram record, one older history word per order, each search within the last match's children.
 CTC_NG_HD float ngram_score(const NgramView &m, const NgramState &in, int32_t w, NgramState &out) {
   const bool probing = m.layout == kNgramKenlmProbing;
+  const bool trie = m.layout == kNgramKenlmTrie;
   float prob = m.uni_prob[w];
   bool stop = probing && (ngram_bits(prob) >> 31);
   if (probing) prob = ngram_float(ngram_bits(prob) | 0x80000000u);
@@ -163,12 +254,22 @@ CTC_NG_HD float ngram_score(const NgramView &m, const NgramState &in, int32_t w,
   out.words[0] = w;
   int matched = 1;
   int32_t key[kNgramMaxOrder];
+  uint32_t lo = 0, hi = 0;  // trie: the children of the longest match so far
+  if (trie && in.len > 0) {
+    const uint64_t u = m.trie.orders[0].bit + 128 * (uint64_t)w + 64;  // (the `next` field of w's unigram record)
+    lo = (uint32_t)ngram_trie_read(m.trie.bits, u);
+    hi = (uint32_t)ngram_trie_read(m.trie.bits, u + 128);
+  }
   for (int j = 0; j < in.len && !stop; ++j) {  // the n-gram of the last j + 1 history words and w
     const int n = j + 2;
-    for (int i = 0; i <= j; ++i) key[i] = in.words[j - i];
-    key[j + 1] = w;
     uint32_t p, bo;
-    if (!ngram_lookup(m, key, n, p, bo)) break;
+    if (trie) {
+      if (!ngram_trie_step(m, n, in.words[j], lo, hi, p, bo)) break;
+    } else {
+      for (int i = 0; i <= j; ++i) key[i] = in.words[j - i];
+      key[j + 1] = w;
+      if (!ngram_lookup(m, key, n, p, bo)) break;
+    }
     if (probing) {
       stop = p >> 31;
       if (n < m.order) p |= 0x80000000u;

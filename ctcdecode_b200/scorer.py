@@ -19,7 +19,8 @@ provider is chosen with ``scorer_provider=`` or the environment variable CTCDECO
 
 ``scorer_provider="device"`` (or CTCDECODE_B200_SCORER_PROVIDER=device) needs no provider: ``ArpaScorer`` has the
 library read the model file itself (ctcdec_scorer_create_arpa): ARPA text, or a KenLM binary file of any type KenLM's
-build_binary writes but REST_PROBING (probing, trie, quantized and array-compressed tries).  Its hooks reproduce the
+build_binary writes but REST_PROBING (probing, trie, quantized and array-compressed tries; a probing file's tables and
+a trie file's packed arrays are searched on the device as they are).  Its hooks reproduce the
 reference Scorer over KenLM bit for bit; a model they cannot reproduce exactly (order above 6, REST_PROBING, a damaged
 binary, ...) is refused.
 """
@@ -68,6 +69,12 @@ class ArpaScorer(object):
 
     def dict_size(self):
         return int(self._lib.ctcdec_scorer_dict_size(self.handle))
+
+    def table_bytes(self):
+        """bytes of n-gram data (unigrams and orders >= 2) the model puts in each device's memory"""
+        n = ctypes.c_size_t()
+        _native.check(self._lib.ctcdec_scorer_table_bytes(self.handle, ctypes.byref(n)))
+        return int(n.value)
 
     def reset_params(self, alpha, beta):
         _native.check(self._lib.ctcdec_scorer_reset_params(self.handle, float(alpha), float(beta)))

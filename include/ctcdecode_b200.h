@@ -185,8 +185,9 @@ int ctcdec_scorer_create(const ctcdec_scorer_hooks *hooks, double alpha, double 
  * the same label-to-word front end over tables of the labels' bytes and the unigrams' spellings.
  * KenLM binary files (format version 5, as build_binary writes them): PROBING files keep their own hash tables, which
  * go to the device byte for byte and are searched there as KenLM searches them; TRIE, QUANT_TRIE, ARRAY_TRIE and
- * QUANT_ARRAY_TRIE files are unpacked on load into the ARPA tables, with the values KenLM reads from the file
- * (dequantized with the file's own bins), at 32 bytes per n-gram in device memory.  The word ids are the file's.
+ * QUANT_ARRAY_TRIE files keep their search data (bit-packed word ids, values and next pointers, Bhiksha offset arrays,
+ * quantization bins) byte for byte too, and the device walks the trie as KenLM's TrieSearch does, reading the values
+ * KenLM reads (dequantized with the file's own bins).  The word ids are the file's.
  * Refused with CTCDEC_E_UNSUPPORTED, the reason in ctcdec_last_error(), anything the tables cannot reproduce exactly:
  * ARPA text: non-ARPA input, order 1 or above 6, counts that disagree with the sections, a malformed line, a duplicate
  * entry, an n-gram word missing from the unigrams, no <s> or </s>, an n-gram whose context is missing, a positive
@@ -198,6 +199,11 @@ int ctcdec_scorer_create(const ctcdec_scorer_hooks *hooks, double alpha, double 
  * CTCDEC_E_INVALID. */
 int ctcdec_scorer_create_arpa(const char *path, double alpha, double beta, const char *const *labels, int n_labels,
                               void **scorer);
+/* Diagnostic: *bytes = the bytes of a scorer from ctcdec_scorer_create_arpa's n-gram data that go to each device it
+ * decodes on: the unigrams and the orders >= 2 (ARPA text: 32-byte entries, two or more slots per n-gram; a probing
+ * file: its own tables; a trie file: its search data), not the dictionary or the front end's tables.  Needs no device.
+ * A hook scorer is CTCDEC_E_UNSUPPORTED. */
+int ctcdec_scorer_table_bytes(const void *scorer, size_t *bytes);
 /* Diagnostic: the scorer's hooks on one label-id prefix -- cond_log_prob and sent_log_prob of ctcdec_scorer_hooks, for a
  * hook scorer or an ARPA scorer.  Labels must lie in [0, n_labels). */
 int ctcdec_scorer_cond_log_prob(const void *scorer, const int32_t *labels, int n, double *out);
