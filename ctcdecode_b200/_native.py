@@ -65,6 +65,11 @@ _SIGNATURES = {
     "ctcdec_decode_batch_lm_device_async": (ctypes.c_int, [ctypes.POINTER(Config), _vp, _vp, ctypes.c_int, _vp,
                                                            ctypes.c_int, ctypes.c_int, _vp, _vp, _vp, _vp, _vp, _vp,
                                                            _vp, _vp, ctypes.c_size_t, _vp]),
+    "ctcdec_lm_sweep_workspace_bytes": (ctypes.c_int, [ctypes.POINTER(Config), _vp, ctypes.c_int, ctypes.c_int,
+                                                       ctypes.c_int, ctypes.POINTER(ctypes.c_size_t)]),
+    "ctcdec_decode_batch_lm_sweep_async": (ctypes.c_int, [ctypes.POINTER(Config), _vp, _vp, ctypes.c_int, _vp,
+                                                          ctypes.c_int, ctypes.c_int, _vp, _vp, ctypes.c_int, _vp, _vp,
+                                                          _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_size_t, _vp]),
     "ctcdec_scorer_rescore_rows": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                                   ctypes.c_int]),
     "ctcdec_state_create":(ctypes.c_int, [ctypes.POINTER(Config), ctypes.c_int, ctypes.POINTER(_vp)]),

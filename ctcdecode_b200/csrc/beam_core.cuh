@@ -288,6 +288,11 @@ struct BeamParams {
   const int *label_word;            // character-based: [V] the word id of each label
   int lm_hist_n;                    // order - 1
   int *lm_hist;                     // [B][arena_stride][order - 1] the node's last order - 1 LM word ids, oldest first
+  // sweep of the LM weights (ctcdec_decode_batch_lm_sweep_async): CTA g decodes input row g % sweep_B (lp, idx,
+  // seq_lens) with the pair lm_ab[g / sweep_B] = (alpha, beta) in place of lm_alpha / beta; everything else is indexed
+  // by g.  sweep_B = 0 (and lm_ab = NULL): CTA g decodes row g with lm_alpha / beta.
+  int sweep_B;
+  const double *lm_ab;              // [P][2]
 };
 
 // control words: 32 ints in L.ctl
@@ -296,7 +301,9 @@ enum {
   C_SMAX, C_NEFREE, C_NETAKEN, C_NRVWORK, C_OVF, C_ANYREF, C_NLIVE, C_SMIN, C_NCAND,
   // second copies, used by frames of odd parity in kernels whose frames have no barrier between reading and
   // resetting these words (beam_program.cuh, "merged front / barrier-free back half")
-  C_OVF_B, C_ANYREF_B, C_NPAIRS_B
+  C_OVF_B, C_ANYREF_B, C_NPAIRS_B,
+  // scorer kernels: the CTA's (alpha, beta) as two doubles in words [C_AB, C_AB + 4) (8-byte aligned: H_CTL is)
+  C_AB = 26
 };
 
 // ---- small helpers --------------------------------------------------------------------------------
@@ -421,7 +428,7 @@ struct Cta {
   uint32_t *s_dmask;    // [KP][WC]: which characters the dictionary lets follow each member
   int WC;
   int space_id;
-  double beta;
+  const double *s_ab;      // this CTA's (alpha, beta) in s_ctl: BeamParams::lm_alpha / beta, or its pair of a sweep
   bool lm_full;
   float lm_cutoff;
   bool lm_char;            // character-based model: no dictionary, an LM term per (member, character)
@@ -435,7 +442,7 @@ struct Cta {
   // language model term when the appended character is the space (reference :120-137): log_p += score; log_p += beta
   CTC_MFN float lm_apply(float log_p, int i) const {
     const float a = f_add(log_p, s_lmsp[i]);
-    return (float)d_add((double)a, beta);
+    return (float)d_add((double)a, s_ab[1]);
   }
   // does appending character ch to member i take a language-model term?  (reference :120: the space of a word-based
   // model, every character of a character-based one)
@@ -444,7 +451,7 @@ struct Cta {
   CTC_MFN float lm_apply_c(float log_p, int i, int ch) const {
     const float term = lm_char ? ld_cg(&lm_row[(size_t)s_node[i] * V + ch]) : s_lmsp[i];
     const float a = f_add(log_p, term);
-    return (float)d_add((double)a, beta);
+    return (float)d_add((double)a, s_ab[1]);
   }
 
   // Score of candidate (beam slot i) + (pruned entry r); false if it is not a new-prefix candidate.

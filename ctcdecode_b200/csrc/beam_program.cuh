@@ -42,19 +42,20 @@ namespace ctc {
 // every child shifts in its character's word id; any other child keeps its parent's history.  The terms are those the
 // host hooks give (lm_host.h lm_after_frame / lm_char_row): float(cond_log_prob * alpha) of history + the node's word
 // (word-based, when a space can follow the node) or of history + each label (character-based, the node's row).
-CTC_FN float lm_dev_term(const BeamParams &p, int *ids, int word) {
+// alpha: the CTA's weight (BeamParams::lm_alpha, or its pair of a sweep).
+CTC_FN float lm_dev_term(const BeamParams &p, double alpha, int *ids, int word) {
   ids[p.lm_hist_n] = word;
-  return (float)(ngram_cond_ids(p.ngram, ids, p.lm_hist_n + 1) * p.lm_alpha);
+  return (float)(ngram_cond_ids(p.ngram, ids, p.lm_hist_n + 1) * alpha);
 }
 
-CTC_FN void lm_dev_root_term(const BeamParams &p, float *lm_row, int c) {
+CTC_FN void lm_dev_root_term(const BeamParams &p, double alpha, float *lm_row, int c) {
   int ids[kNgramMaxOrder];
   for (int k = 0; k < p.lm_hist_n; ++k) ids[k] = p.ngram.bos;
-  lm_row[c] = lm_dev_term(p, ids, p.label_word[c]);
+  lm_row[c] = lm_dev_term(p, alpha, ids, p.label_word[c]);
 }
 
-CTC_FN void lm_dev_node(const BeamParams &p, int *hist, float *lm_arena, float *lm_row, int nid, int par, int ch,
-                        int par_state, int arc, int dst) {
+CTC_FN void lm_dev_node(const BeamParams &p, double alpha, int *hist, float *lm_arena, float *lm_row, int nid, int par,
+                        int ch, int par_state, int arc, int dst) {
   const int H = p.lm_hist_n;
   int ids[kNgramMaxOrder];
   const int *hp = hist + (size_t)par * H;
@@ -63,9 +64,9 @@ CTC_FN void lm_dev_node(const BeamParams &p, int *hist, float *lm_arena, float *
   if (shift) ids[H - 1] = p.lm_char ? p.label_word[ch] : p.word_of_state[par_state];
   for (int k = 0; k < H; ++k) hist[(size_t)nid * H + k] = ids[k];
   if (p.lm_char) {
-    for (int c = 0; c < p.V; ++c) lm_row[(size_t)nid * p.V + c] = lm_dev_term(p, ids, p.label_word[c]);
+    for (int c = 0; c < p.V; ++c) lm_row[(size_t)nid * p.V + c] = lm_dev_term(p, alpha, ids, p.label_word[c]);
   } else if (arc & kDictSpace) {
-    lm_arena[nid] = lm_dev_term(p, ids, p.word_of_state[dst]);
+    lm_arena[nid] = lm_dev_term(p, alpha, ids, p.word_of_state[dst]);
   }
 }
 
@@ -403,7 +404,11 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
   c.K = K; c.KP = KP; c.V = V; c.NP = NP; c.W = W; c.blank = p.blank;
   c.WS = WS; c.mch = MERGED;
   c.s_dmask = (uint32_t *)(smem + L.dmask); c.WC = L.WC;
-  c.dict_next = p.dict_next; c.space_id = p.space_id; c.beta = p.beta; c.lm_full = false; c.lm_cutoff = kNInf;
+  c.dict_next = p.dict_next; c.space_id = p.space_id; c.lm_full = false; c.lm_cutoff = kNInf;
+  c.s_ab = (const double *)(smem + H_CTL + C_AB * 4);
+  // sweep of the LM weights: the input row of this CTA, and its (alpha, beta) pair (read once, at the start)
+  const int bi = LM && p.sweep_B ? b % p.sweep_B : b;
+  const double *const lm_pair = LM && p.lm_ab ? p.lm_ab + 2 * (b / p.sweep_B) : nullptr;
   c.lm_char = LM && p.lm_char != 0; c.lm_row = nullptr;
   int *const s_ctl = c.s_ctl;
 #if !defined(CTC_EMULATE)
@@ -501,7 +506,7 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
     }
 #endif
   };
-  int Tb = p.seq_lens ? p.seq_lens[b] : p.T;  // reference binding.cpp:64-65 clamps to T
+  int Tb = p.seq_lens ? p.seq_lens[bi] : p.T;  // reference binding.cpp:64-65 clamps to T
   if (Tb > p.T) Tb = p.T;
   const int t0 = p.nframes > 0 ? p.t0 : 0;
   Tb -= t0;
@@ -570,6 +575,11 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
       s_ctl[C_M] = fresh ? 1 : st[0];
       s_ctl[C_NNODES] = fresh ? 1 : st[1];
       s_ctl[C_FLAGS] = fresh ? 0 : st[3];
+      if (LM) {
+        double *const ab = (double *)(s_ctl + C_AB);
+        ab[0] = lm_pair ? lm_pair[0] : p.lm_alpha;
+        ab[1] = lm_pair ? lm_pair[1] : p.beta;
+      }
       s_ctl[C_KMIN] = (int)0xFFFFFFFFu;
       s_ctl[C_SMIN] = (int)0xFFFFFFFFu;
       if (fresh) {  // root node (reference path_trie.cpp:11-30)
@@ -583,15 +593,15 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
     if (LM && p.lm_dev && abs_t0 == 0) {
       for (int k = tid; k < p.lm_hist_n; k += NT) lm_hist[k] = p.ngram.bos;
       if (p.lm_char)
-        for (int x = tid; x < V; x += NT) lm_dev_root_term(p, lm_row, x);
+        for (int x = tid; x < V; x += NT) lm_dev_root_term(p, lm_pair ? lm_pair[0] : p.lm_alpha, lm_row, x);
     }
   }
 #if !defined(CTC_EMULATE)
   uint64_t *const mbar = (uint64_t *)(smem + H_MBAR);
   float *const tile_lp = (float *)(smem + L.tile_lp);
   uint16_t *const tile_idx = (uint16_t *)(smem + L.tile_idx);
-  const float *const g_lp = p.lp + ((size_t)b * p.T + t0) * NP;
-  const uint16_t *const g_idx = SORTED ? p.idx + ((size_t)b * p.T + t0) * NP : nullptr;
+  const float *const g_lp = p.lp + ((size_t)bi * p.T + t0) * NP;
+  const uint16_t *const g_idx = SORTED ? p.idx + ((size_t)bi * p.T + t0) * NP : nullptr;
   if (threadIdx.x == 0) {
     mbar_init(&mbar[0], 1);
     mbar_init(&mbar[1], 1);
@@ -656,8 +666,8 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
   for (int t = 0; t < Tb; ++t) {
     const int t_abs = abs_t0 + t;
 #if defined(CTC_EMULATE)
-    c.lp = p.lp + ((size_t)b * p.T + t0 + t) * NP;
-    c.idx = SORTED ? p.idx + ((size_t)b * p.T + t0 + t) * NP : nullptr;
+    c.lp = p.lp + ((size_t)bi * p.T + t0 + t) * NP;
+    c.idx = SORTED ? p.idx + ((size_t)bi * p.T + t0 + t) * NP : nullptr;
 #else
     {
       if (ft == F) { ft = 0; ++tile; }
@@ -764,7 +774,7 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
       }
       CTC_BARRIER();
       const float worst = unord_f((unsigned)s_ctl[C_SMIN]);
-      const double mx0 = p.beta > 0.0 ? p.beta : 0.0;
+      const double mx0 = c.s_ab[1] > 0.0 ? c.s_ab[1] : 0.0;
       c.lm_full = (M == K);
       c.lm_cutoff = (float)d_add((double)f_add(worst, c.lp[NP - 3]), -mx0);
     }
@@ -1239,7 +1249,10 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
       if (LM) {
         lo32 = (!select_all && M == K) ? (unsigned)s_ctl[C_KMIN] : 0u;
         top32 = (unsigned)s_ctl[C_KMAX];
-        const unsigned o = ord_f(f_add(unord_f((unsigned)s_ctl[C_SMAX]), lpmax));
+        // a scored candidate gains its LM term (<= 0) and beta: with beta > 0 it can end above the best member score
+        // plus the row's best log-prob, by at most beta (its key outside the range would index past the histogram)
+        const double bmax = c.s_ab[1] > 0.0 ? c.s_ab[1] : 0.0;
+        const unsigned o = ord_f((float)d_add((double)f_add(unord_f((unsigned)s_ctl[C_SMAX]), lpmax), bmax));
         top32 = o > top32 ? o : top32;
         set_shift();
       }
@@ -1317,8 +1330,8 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
     //      the tile was requested a whole tile ago), into the table the members' region of this frame cleared
     if (MERGED && SORTED && t + 1 < Tb) {
 #if defined(CTC_EMULATE)
-      const float *nrow = p.lp + ((size_t)b * p.T + t0 + t + 1) * NP;
-      const uint16_t *nidx = p.idx + ((size_t)b * p.T + t0 + t + 1) * NP;
+      const float *nrow = p.lp + ((size_t)bi * p.T + t0 + t + 1) * NP;
+      const uint16_t *nidx = p.idx + ((size_t)bi * p.T + t0 + t + 1) * NP;
 #else
       int ft2 = ft, tile2 = tile;
       if (ft2 == F) { ft2 = 0; ++tile2; mbar_wait(&mbar[tile2 & 1], (uint32_t)((tile2 >> 1) & 1)); }
@@ -1560,7 +1573,7 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
           }
           const unsigned nmin = ctc_warp_min(kmn), nmax = ctc_warp_max(kmx);
 #if defined(CTC_EMULATE)
-          const float *nrow = p.lp + ((size_t)b * p.T + t0 + t + 1) * NP;
+          const float *nrow = p.lp + ((size_t)bi * p.T + t0 + t + 1) * NP;
 #else
           int ft2 = ft, tile2 = tile;
           if (ft2 == F) { ft2 = 0; ++tile2; mbar_wait(&mbar[tile2 & 1], (uint32_t)((tile2 >> 1) & 1)); }

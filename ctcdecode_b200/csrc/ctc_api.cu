@@ -99,18 +99,49 @@ __global__ void stream_table_kernel(const StreamTabArgs a) {
   reinterpret_cast<int *>(a.tab + a.L.lens)[b] = a.len[i];
 }
 
+// The (alpha, beta) pairs of a sweep (ctcdec_decode_batch_lm_sweep_async) into the workspace, from the launch parameters
+// (kTabPerLaunch pairs per launch), so that the call copies nothing from host memory and a graph replays the pairs it
+// captured.
+struct SweepPairArgs {
+  double *tab;
+  int p0, n;
+  double ab[2 * kTabPerLaunch];
+};
+__global__ void sweep_pairs_kernel(const SweepPairArgs a) {
+  const int i = (int)threadIdx.x;
+  if (i >= a.n) return;
+  a.tab[2 * (a.p0 + i)] = a.ab[2 * i];
+  a.tab[2 * (a.p0 + i) + 1] = a.ab[2 * i + 1];
+}
+
+// Sweep: the prune scan's flags of the B input rows (slice 0 of flags [P][B]) into the other P - 1 slices, before the
+// beam and finalize kernels OR in each CTA's own bits.
+__global__ void sweep_flags_kernel(int32_t *flags, int B, long long n) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) flags[B + i] = flags[i % B];
+}
+
 // Read-out of an ARPA scorer's results (ngram_readout_row, reference DecoderState::decode): one thread per [B, K] result
 // row, rows p >= n_results[b] skipped, scores rescored in place.  Each row is a serial chain of hash probes (about
-// words x order of them).
+// words x order of them).  SWEEP: row r takes the pair ab[r / (pair_B x K)] instead of alpha / beta.  (A compile-time
+// choice: the two doubles loaded per row stay live across the row's walks and cost the kernel a spill, which the
+// single-pair instantiation is kept free of.)
 constexpr int kReadoutThreads = 128;
+template <bool SWEEP>
 __global__ void __launch_bounds__(kReadoutThreads) lm_readout_kernel(const NgramView m, const NgramFront f, double alpha,
-                                                                     double beta, const int32_t *tokens,
+                                                                     double beta, const double *ab, int pair_B,
+                                                                     const int32_t *tokens,
                                                                      const int32_t *lens, const int32_t *n_results,
                                                                      float *scores, int B, int K, int row_stride) {
   const long long r = (long long)blockIdx.x * kReadoutThreads + threadIdx.x;
   if (r >= (long long)B * K) return;
   const int b = (int)(r / K), p = (int)(r % K);
   if (p >= n_results[b]) return;
+  if (SWEEP) {
+    const int q = b / pair_B;
+    alpha = ab[2 * q];
+    beta = ab[2 * q + 1];
+  }
   scores[r] = ngram_readout_row(m, f, tokens + r * row_stride, lens[r], scores[r], alpha, beta);
 }
 
@@ -548,13 +579,20 @@ static int ensure_ngram_on_device(HostScorer *sc, int device) {
 }
 
 // Enqueues the read-out of an ARPA scorer's [B, K] result rows (row_stride columns each) on s; the scorer's tables must
-// be on the current device.  alpha and beta are the scorer's values now.
+// be on the current device.  alpha and beta are the scorer's values now, or, for a sweep, the device table ab [P][2]
+// with pair_B utterances per pair.
 static int launch_readout(const HostScorer *sc, const int32_t *tokens, const int32_t *lens, const int32_t *n_results,
-                          float *scores, int B, int K, int row_stride, cudaStream_t s) {
+                          float *scores, int B, int K, int row_stride, cudaStream_t s, const double *ab = nullptr,
+                          int pair_B = 0) {
   const long long rows = (long long)B * K;
   if (rows == 0) return CTCDEC_OK;
-  lm_readout_kernel<<<(unsigned)((rows + kReadoutThreads - 1) / kReadoutThreads), kReadoutThreads, 0, s>>>(
-      sc->d_view, sc->d_front, sc->alpha, sc->beta, tokens, lens, n_results, scores, B, K, row_stride);
+  const unsigned grid = (unsigned)((rows + kReadoutThreads - 1) / kReadoutThreads);
+  if (ab)
+    lm_readout_kernel<true><<<grid, kReadoutThreads, 0, s>>>(sc->d_view, sc->d_front, 0.0, 0.0, ab, pair_B, tokens,
+                                                             lens, n_results, scores, B, K, row_stride);
+  else
+    lm_readout_kernel<false><<<grid, kReadoutThreads, 0, s>>>(sc->d_view, sc->d_front, sc->alpha, sc->beta, nullptr,
+                                                              1, tokens, lens, n_results, scores, B, K, row_stride);
   CU(cudaGetLastError());
   return CTCDEC_OK;
 }
@@ -1550,6 +1588,10 @@ struct LmBuffers {
   int32_t *tokens, *timesteps;   // [B, K, T]
   float *scores;                 // [B, K] (the raw prefix scores: the caller rescores them with lm_rescore_batch)
   int32_t *lens, *n_results, *flags;
+  // sweep of the LM weights (ARPA scorer): P pairs (alpha, beta) in the device table lm_ab [P][2]; the per-node arrays
+  // and the outputs above then hold P x B utterances (pair-major), the input rows B
+  int P = 1;
+  const double *lm_ab = nullptr;
 };
 
 // One offline scorer decode from the point where the input is on the device, enqueued on s; shared by both scorer
@@ -1565,10 +1607,16 @@ static int lm_batch_step(const ctcdec_config *cfg, const Plan &pl, HostScorer *s
   int rc = ensure_dict_on_device(sc, device);
   if (rc || (sc->ngram && (rc = ensure_ngram_on_device(sc, device)))) return rc;
   const bool lm_char = sc->is_character_based != 0;
-  CU(cudaMemsetAsync(io.flags, 0, (size_t)B * 4, s));
+  const int G = io.P * B;  // beam CTAs
+  CU(cudaMemsetAsync(io.flags, 0, (size_t)G * 4, s));
   float *lp = reinterpret_cast<float *>(io.ws + pl.off_lp);
   uint16_t *idx = pl.sorted ? reinterpret_cast<uint16_t *>(io.ws + pl.off_idx) : nullptr;
   if ((rc = launch_prune(cfg, pl, io.in, io.seq_lens, B, T, lp, idx, io.flags, s))) return rc;
+  if (io.P > 1) {
+    const long long n = (long long)(io.P - 1) * B;
+    sweep_flags_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(io.flags, B, n);
+    CU(cudaGetLastError());
+  }
 
   BeamParams bp;
   memset(&bp, 0, sizeof(bp));
@@ -1590,9 +1638,10 @@ static int lm_batch_step(const ctcdec_config *cfg, const Plan &pl, HostScorer *s
     bp.lm_dev = 1; bp.lm_alpha = sc->alpha; bp.ngram = sc->d_view;
     bp.word_of_state = sc->d_word_of_state; bp.label_word = sc->d_label_word;
     bp.lm_hist_n = sc->max_order - 1; bp.lm_hist = io.lm_hist;
+    bp.sweep_B = io.lm_ab ? B : 0; bp.lm_ab = io.lm_ab;
     bp.t0 = 0; bp.nframes = 0; bp.fresh = 1;
-    if ((rc = launch_beam(bp, pl, B, s))) return rc;
-    return launch_finalize(bp, B, s);
+    if ((rc = launch_beam(bp, pl, G, s))) return rc;
+    return launch_finalize(bp, G, s);
   }
   int nls = 0, ups = 0;
   exchange_strides(K, exchange_row_len(*sc), &nls, &ups);
@@ -1818,6 +1867,38 @@ int ctcdec_lm_workspace_bytes(const ctcdec_config *cfg, const void *scorer, int 
   return CTCDEC_OK;
 }
 
+// A sweep of P (alpha, beta) pairs over B utterances: the launch plan of a B-utterance decode (its block size: the
+// 128- and 256-thread kernels can order comparator-equal results differently, and slice p must equal that decode bit
+// for bit; with a scorer both keep two CTAs per SM), the arenas, states and per-node arrays of P x B beam CTAs, the
+// pruned rows of the B input utterances (scanned once), and the device table of the pairs at w->total (*bytes: the
+// whole workspace the caller provides).
+static int lm_sweep_plan(const ctcdec_config *cfg, const void *scorer, int B, int T, int P, Plan *pl, LmWorkspace *w,
+                         size_t *bytes) {
+  if (P < 1) return fail(CTCDEC_E_INVALID, "%d (alpha, beta) pairs: a sweep needs at least one", P);
+  if (B > 0 && (long long)P * B > 0x7fffffffll)
+    return fail(CTCDEC_E_UNSUPPORTED, "%d pairs x batch %d: too many beam CTAs", P, B);
+  if (scorer && !static_cast<const HostScorer *>(scorer)->ngram)
+    return fail(CTCDEC_E_UNSUPPORTED, "a sweep takes a scorer from ctcdec_scorer_create_arpa only: a hook scorer's "
+                "terms float(cond_log_prob x alpha) are computed on the host");
+  int rc = lm_device_plan(cfg, scorer, B, T, pl, w);
+  if (rc) return rc;
+  plan_regions(pl, B, P * B, T);
+  if ((rc = lm_workspace(static_cast<const HostScorer *>(scorer), *pl, P * B, w))) return rc;
+  *bytes = w->total + al256((size_t)P * 16) + 256;
+  return CTCDEC_OK;
+}
+
+int ctcdec_lm_sweep_workspace_bytes(const ctcdec_config *cfg, const void *scorer, int B, int T, int P, size_t *bytes) {
+  Plan pl;
+  LmWorkspace w;
+  size_t need = 0;
+  const int rc = lm_sweep_plan(cfg, scorer, B, T, P, &pl, &w, &need);
+  if (rc) return rc;
+  if (!bytes) return fail(CTCDEC_E_INVALID, "bytes is NULL");
+  *bytes = need;
+  return CTCDEC_OK;
+}
+
 int ctcdec_decode_batch_lm_device(const ctcdec_config *cfg, void *scorer, const void *input, int dtype,
                                   const int32_t *seq_lens, int B, int T, int32_t *tokens, int32_t *timesteps,
                                   float *scores, int32_t *lens, int32_t *n_results, int32_t *flags,
@@ -1899,23 +1980,29 @@ int ctcdec_decode_batch_lm_device(const ctcdec_config *cfg, void *scorer, const 
   return check_error_flags(h_flags, B);
 }
 
-int ctcdec_decode_batch_lm_device_async(const ctcdec_config *cfg, void *scorer, const void *input, int dtype,
-                                        const int32_t *seq_lens, int B, int T, int32_t *tokens, int32_t *timesteps,
-                                        float *scores, int32_t *lens, int32_t *n_results, int32_t *flags,
-                                        float *log_probs_out, void *workspace, size_t workspace_bytes, void *stream) {
+// ctcdec_decode_batch_lm_device_async (P = 0: the scorer's alpha and beta) and ctcdec_decode_batch_lm_sweep_async (P >= 1
+// host pairs: outputs [P, B, ...]).
+static int lm_decode_async(const ctcdec_config *cfg, void *scorer, const void *input, int dtype,
+                           const int32_t *seq_lens, int B, int T, const double *alphas, const double *betas, int P,
+                           int32_t *tokens, int32_t *timesteps, float *scores, int32_t *lens, int32_t *n_results,
+                           int32_t *flags, float *log_probs_out, void *workspace, size_t workspace_bytes, void *stream) {
   if (!scorer) return fail(CTCDEC_E_INVALID, "scorer is NULL");
   if (dtype != -1 && dtype != CTCDEC_DTYPE_F32 && dtype != CTCDEC_DTYPE_F16 && dtype != CTCDEC_DTYPE_BF16)
     return fail(CTCDEC_E_INVALID, "dtype %d is not -1 (probabilities) or one of CTCDEC_DTYPE_F32 / F16 / BF16", dtype);
   const int kind = dtype == -1 ? IN_F32 : dtype == CTCDEC_DTYPE_F32 ? IN_LOGITS_F32
                  : dtype == CTCDEC_DTYPE_F16 ? IN_LOGITS_F16 : IN_LOGITS_BF16;
+  const bool sweep = P > 0;
   Plan pl;
   LmWorkspace w;
-  int rc = lm_device_plan(cfg, scorer, B, T, &pl, &w);
+  size_t need_bytes = 0;
+  int rc = sweep ? lm_sweep_plan(cfg, scorer, B, T, P, &pl, &w, &need_bytes) : lm_device_plan(cfg, scorer, B, T, &pl, &w);
   if (rc) return rc;
+  if (!sweep) need_bytes = w.total + 256;
   HostScorer *sc = static_cast<HostScorer *>(scorer);
   if (!sc->ngram)
     return fail(CTCDEC_E_UNSUPPORTED, "the asynchronous scorer decode takes a scorer from ctcdec_scorer_create_arpa only: "
                 "a hook scorer needs the host during the call (use ctcdec_decode_batch_lm_device)");
+  if (sweep && (!alphas || !betas)) return fail(CTCDEC_E_INVALID, "alphas and betas (host double[P]) are required");
   if (B > 0 && (!n_results || !flags)) return fail(CTCDEC_E_INVALID, "n_results and flags device buffers are required");
   if (B > 0 && (!scores || !lens || (T > 0 && (!input || !tokens || !timesteps))))
     return fail(CTCDEC_E_INVALID, "the input or an output pointer is NULL");
@@ -1924,7 +2011,6 @@ int ctcdec_decode_batch_lm_device_async(const ctcdec_config *cfg, void *scorer, 
   CU(cudaGetDevice(&device));
   if (device >= 64) return fail(CTCDEC_E_INVALID, "device %d out of range", device);
   if (B == 0) return CTCDEC_OK;
-  const size_t need_bytes = w.total + 256;
   if (!workspace || workspace_bytes < need_bytes)
     return fail(CTCDEC_E_WORKSPACE, "workspace of %zu bytes given, %zu needed", workspace_bytes, need_bytes);
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
@@ -1951,9 +2037,42 @@ int ctcdec_decode_batch_lm_device_async(const ctcdec_config *cfg, void *scorer, 
   io.lm_hist = reinterpret_cast<int *>(ws + w.hist);
   io.tokens = tokens; io.timesteps = timesteps; io.scores = scores; io.lens = lens; io.n_results = n_results;
   io.flags = flags;
+  if (sweep) {
+    // each pair through float32, as ctcdec_scorer_reset_params stores them
+    double *tab = reinterpret_cast<double *>(ws + w.total);
+    for (int p0 = 0; p0 < P; p0 += kTabPerLaunch) {
+      SweepPairArgs a;
+      a.tab = tab; a.p0 = p0; a.n = std::min(kTabPerLaunch, P - p0);
+      for (int i = 0; i < a.n; ++i) {
+        a.ab[2 * i] = (double)(float)alphas[p0 + i];
+        a.ab[2 * i + 1] = (double)(float)betas[p0 + i];
+      }
+      sweep_pairs_kernel<<<1, kTabPerLaunch, 0, s>>>(a);
+      CU(cudaGetLastError());
+    }
+    io.P = P; io.lm_ab = tab;
+  }
   // (the host lengths only serve the hook scorers' handshake: the ARPA branch of the step reads the device copy)
   if ((rc = lm_batch_step(cfg, pl, sc, g_cache[device], device, nullptr, B, T, io, s))) return rc;
-  return launch_readout(sc, tokens, lens, n_results, scores, B, cfg->beam_size, T, s);
+  return launch_readout(sc, tokens, lens, n_results, scores, io.P * B, cfg->beam_size, T, s, io.lm_ab, B);
+}
+
+int ctcdec_decode_batch_lm_device_async(const ctcdec_config *cfg, void *scorer, const void *input, int dtype,
+                                        const int32_t *seq_lens, int B, int T, int32_t *tokens, int32_t *timesteps,
+                                        float *scores, int32_t *lens, int32_t *n_results, int32_t *flags,
+                                        float *log_probs_out, void *workspace, size_t workspace_bytes, void *stream) {
+  return lm_decode_async(cfg, scorer, input, dtype, seq_lens, B, T, nullptr, nullptr, 0, tokens, timesteps, scores,
+                         lens, n_results, flags, log_probs_out, workspace, workspace_bytes, stream);
+}
+
+int ctcdec_decode_batch_lm_sweep_async(const ctcdec_config *cfg, void *scorer, const void *input, int dtype,
+                                       const int32_t *seq_lens, int B, int T, const double *alphas,
+                                       const double *betas, int P, int32_t *tokens, int32_t *timesteps, float *scores,
+                                       int32_t *lens, int32_t *n_results, int32_t *flags, float *log_probs_out,
+                                       void *workspace, size_t workspace_bytes, void *stream) {
+  if (P < 1) return fail(CTCDEC_E_INVALID, "%d (alpha, beta) pairs: a sweep needs at least one", P);
+  return lm_decode_async(cfg, scorer, input, dtype, seq_lens, B, T, alphas, betas, P, tokens, timesteps, scores, lens,
+                         n_results, flags, log_probs_out, workspace, workspace_bytes, stream);
 }
 
 // Diagnostic: the read-out of [B, K] host rows, on the host (lm_rescore_batch through the scorer's hooks) or by the

@@ -46,6 +46,17 @@ static inline PruneShape prune_shape(const Plan &pl, int V, bool logits) {
   return PruneShape{wpc, 2048 + (size_t)wpc * per_warp};
 }
 
+// Workspace carve-up: the pruned rows of `rows` input utterances, then the node arenas and state blocks of `ctas` beam
+// CTAs (the same number except in a sweep of the LM weights, where P pairs decode each input row).
+static inline void plan_regions(Plan *pl, int rows, int ctas, int T) {
+  size_t o = 0;
+  pl->off_lp = o;     o = al256(o + (size_t)rows * T * pl->NP * 4);
+  pl->off_idx = o;    o = al256(o + (pl->sorted ? (size_t)rows * T * pl->NP * 2 : 0));
+  pl->off_arena = o;  o = al256(o + (size_t)ctas * pl->arena_stride * sizeof(Node));
+  pl->off_state = o;  o = al256(o + (size_t)ctas * pl->state_stride * 4);
+  pl->total = o;
+}
+
 // b_sched: the number of utterances that will be in flight on the device together (>= B when the caller runs
 // several groups of B concurrently); decides between the latency and the throughput shape of the beam kernel.
 // lm: a scorer is attached.  Its beam kernel carries the [KP][WC] dictionary masks as well (make_layout(..., lm =
@@ -98,12 +109,7 @@ static inline int make_plan_core(const ctcdec_config *cfg, int B, int T, Plan *p
     PLAN_FAIL(CTCDEC_E_UNSUPPORTED, "vocab_size %d too large for the in-shared-memory vocabulary sort (at most 16384)", V);
   pl->arena_stride = 1 + (long long)K * T;
   pl->state_stride = (state_ints(K) + 63) / 64 * 64;
-  size_t o = 0;
-  pl->off_lp = o;     o = al256(o + (size_t)B * T * pl->NP * 4);
-  pl->off_idx = o;    o = al256(o + (pl->sorted ? (size_t)B * T * pl->NP * 2 : 0));
-  pl->off_arena = o;  o = al256(o + (size_t)B * pl->arena_stride * sizeof(Node));
-  pl->off_state = o;  o = al256(o + (size_t)B * pl->state_stride * 4);
-  pl->total = o;
+  plan_regions(pl, B, B, T);
   msg[0] = 0;
   return CTCDEC_OK;
 #undef PLAN_FAIL

@@ -29,6 +29,8 @@ Differences from the reference, all additive:
     call may return before the results exist, and a kernel error shows only as CTCDEC_FLAG_ERR_ARENA in
     ``last_flags``, a CUDA tensor.  ``OnlineCTCBeamDecoder`` then decodes CUDA chunks and ``decode_logits`` with the
     device scorer on the GPU as well.
+  * ``decode_sweep(x, alphas, betas)`` (device scorer): one batch under P (alpha, beta) pairs in one enqueue, results
+    with a leading pair axis, each slice equal to ``decode`` after ``reset_params`` with that pair.
   * the [batch, beam, T] result tensors are PAGE-LOCKED CPU tensors (torch's caching host allocator, so a decode loop
     reuses the same blocks) up to CTCDECODE_B200_PIN_OUTPUT_BYTES per tensor (default 1 GiB), pageable beyond: a fresh
     pageable [256, 100, 1000] int32 pair costs page faults on every call, several times the decode itself.
@@ -299,6 +301,85 @@ class CTCBeamDecoder(_Base):
     def reset_params(self, alpha, beta):
         if self._scorer is not None:  # reference __init__.py:134-136
             self._scorer.reset_params(alpha, beta)
+
+    def decode_sweep(self, x, alphas, betas, seq_lens=None, logits=False):
+        """Extension: decode one batch under P language-model weight pairs (alphas[p], betas[p]) in one enqueue
+        (ctcdec_decode_batch_lm_sweep_async), e.g. to tune alpha and beta on a dev set; a grid is the caller's
+        itertools.product.  x: [B, T, V] probabilities (log-probabilities with log_probs_input), CPU or CUDA, or with
+        logits=True raw float32 / float16 / bfloat16 CUDA logits as in decode_logits.  Returns the four tensors of
+        decode with a leading pair axis -- beam_results / timesteps [P, B, beam, T], beam_scores / out_lens [P, B, beam]
+        -- and sets last_flags / last_n_results [P, B].  Slice p equals decode after reset_params(alphas[p], betas[p])
+        (both rounded to float32, as reset_params does); the decoder's own alpha and beta stay as they are.  CPU input
+        is uploaded and the call waits; CUDA input follows device_outputs / non_blocking as decode does.  Needs the
+        device scorer (scorer_provider="device")."""
+        from .scorer import ArpaScorer
+        if not isinstance(self._scorer, ArpaScorer):
+            raise ValueError('decode_sweep needs a language model with scorer_provider="device": the sweep runs the '
+                             "device n-gram scorer")
+        alphas = [float(a) for a in alphas]
+        betas = [float(b) for b in betas]
+        if len(alphas) != len(betas) or not alphas:
+            raise ValueError("alphas and betas must be non-empty and of equal length, got %d and %d"
+                             % (len(alphas), len(betas)))
+        if x.dim() != 3:
+            raise ValueError("x must be [batch, time, labels], got %s" % (tuple(x.shape),))
+        B, T, V = x.shape
+        if V != self._num_labels:
+            raise ValueError("x has %d labels, decoder was built with %d" % (V, self._num_labels))
+        dtype = -1
+        if logits:
+            dtypes = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
+            if not x.is_cuda or x.dtype not in dtypes:
+                raise ValueError("logits must be a float32, float16 or bfloat16 CUDA tensor")
+            dtype = dtypes[x.dtype]
+            x = x.contiguous()
+        host = not x.is_cuda
+        dev = x.device if not host else torch.device("cuda", self._device_index())
+        if dtype == -1:
+            x = x.to(device=dev, dtype=torch.float32).contiguous()
+        if seq_lens is not None:
+            seq_lens = seq_lens.to(device=dev, dtype=torch.int32).contiguous()
+        lib = _native.load()
+        cfg = _cfg(self)
+        K, P = self._beam_width, len(alphas)
+        scorer = self._scorer.handle
+        nbytes = ctypes.c_size_t(0)
+        _native.check(lib.ctcdec_lm_sweep_workspace_bytes(ctypes.byref(cfg), scorer, B, T, P, ctypes.byref(nbytes)))
+        if self._ws is None or self._ws.numel() < nbytes.value or self._ws.device != dev:
+            self._ws = None
+            self._ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        output = torch.empty(P, B, K, T, dtype=torch.int32, device=dev)
+        timesteps = torch.empty(P, B, K, T, dtype=torch.int32, device=dev)
+        scores = torch.empty(P, B, K, dtype=torch.float32, device=dev)
+        out_seq_len = torch.zeros(P, B, K, dtype=torch.int32, device=dev)
+        n_results = torch.zeros(P, B, dtype=torch.int32, device=dev)
+        flags = torch.zeros(P, B, dtype=torch.int32, device=dev)
+        a = (ctypes.c_double * P)(*alphas)
+        b = (ctypes.c_double * P)(*betas)
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            _native.check(lib.ctcdec_decode_batch_lm_sweep_async(
+                ctypes.byref(cfg), scorer, x.data_ptr(), dtype, seq_lens.data_ptr() if seq_lens is not None else None,
+                B, T, a, b, P, output.data_ptr(), timesteps.data_ptr(), scores.data_ptr(), out_seq_len.data_ptr(),
+                n_results.data_ptr(), flags.data_ptr(), None, self._ws.data_ptr(), self._ws.numel(), stream))
+        self.last_flags, self.last_n_results = flags, n_results
+        if self._device_outputs and not host:
+            if not self._non_blocking:
+                torch.cuda.current_stream(dev).synchronize()
+                self._check_flags(flags)
+            return output, scores, timesteps, out_seq_len
+        torch.cuda.current_stream(dev).synchronize()
+        self._check_flags(flags)
+        self.last_flags, self.last_n_results = flags.cpu(), n_results.cpu()
+        return output.cpu(), scores.cpu(), timesteps.cpu(), out_seq_len.cpu()
+
+    @staticmethod
+    def _check_flags(flags):
+        bad = (flags & _native.FLAG_ERR_ARENA).nonzero()
+        if bad.numel():
+            p, b = (int(v) for v in bad[0])
+            raise _native.NativeError("pair %d, utterance %d: the beam kernel reported an internal error; results are "
+                                      "not valid" % (p, b))
 
 
 class OnlineCTCBeamDecoder(_Base):

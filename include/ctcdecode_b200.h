@@ -286,6 +286,42 @@ int ctcdec_decode_batch_lm_device_async(const ctcdec_config *cfg, void *scorer, 
                                         float *scores, int32_t *lens, int32_t *n_results, int32_t *flags,
                                         float *log_probs_out, void *workspace, size_t workspace_bytes, void *stream);
 
+/* Bytes of device scratch ctcdec_decode_batch_lm_sweep_async needs for P (alpha, beta) pairs over a [B, T, V] batch:
+ * ctcdec_lm_workspace_bytes(cfg, scorer, P x B, T), less the pruned rows of (P - 1) x B utterances (the input is scanned
+ * once: B x T x NP x 4 bytes, and B x T x NP x 2 more when the vocabulary is cut, each region 256-byte aligned; NP is
+ * the pruned row length, min(V, cutoff_top_n) + 3 -- V + 3 without a cut -- rounded up to a multiple of 8), plus the
+ * pairs' table (16 x P bytes, 256-byte aligned).  The 64 GiB limits of the per-node rows and histories apply to the
+ * P x B utterances.  The same refusals as ctcdec_lm_workspace_bytes, no device needed; also CTCDEC_E_INVALID for
+ * P < 1 and CTCDEC_E_UNSUPPORTED for a hook scorer. */
+int ctcdec_lm_sweep_workspace_bytes(const ctcdec_config *cfg, const void *scorer, int B, int T, int P, size_t *bytes);
+
+/* Extension: a sweep of the language-model weights.  Decodes one batch under P pairs (alphas[p], betas[p]), host
+ * double[P] arrays, in one enqueue: the vocabulary scan runs once over the B input utterances, then one beam CTA per
+ * (pair, utterance).  Slice p of every output is exactly what ctcdec_decode_batch_lm_device_async returns for the same
+ * batch after ctcdec_scorer_reset_params(scorer, alphas[p], betas[p]): each value goes through float32, as reset_params
+ * stores it (reference Scorer::reset_params(float, float)), so the baseline is reset_params, not a scorer created with
+ * the unrounded doubles.  The scorer's own alpha and beta are neither read nor changed.
+ *   Arguments as ctcdec_decode_batch_lm_device_async (seq_lens a DEVICE int32 [B] buffer or NULL, log_probs_out
+ *              [B, T, V], written once), except the outputs, all contiguous device buffers with a leading pair axis:
+ *              tokens / timesteps [P, B, beam, T], scores / lens [P, B, beam], n_results / flags [P, B].  Slice p is
+ *              laid out as a B-utterance decode writes it.  flags[p, b] carries the vocabulary scan's
+ *              CTCDEC_FLAG_TIE_VOCAB bit of utterance b and the beam and finalize bits of its own decode.
+ *   Workspace: ctcdec_lm_sweep_workspace_bytes.  The beam kernel runs with the block size a B-utterance decode gets:
+ *              the 128- and 256-thread kernels may order comparator-equal results (CTCDEC_FLAG_TIE_FINAL) differently.
+ *   CUDA graphs: as ctcdec_decode_batch_lm_device_async -- decode once outside the capture first.  After its checks the
+ *              call copies nothing from pageable or pinned host memory: the pairs travel in kernel launch parameters,
+ *              so a graph replays the pairs it captured.
+ *   Errors of the kernels show in flags only: a set CTCDEC_FLAG_ERR_ARENA means that (pair, utterance)'s results are
+ *              not valid.
+ * A scorer from ctcdec_scorer_create_arpa only (word- or character-based, ARPA text or a KenLM binary); a hook scorer
+ * returns CTCDEC_E_UNSUPPORTED (its terms float(cond_log_prob x alpha) are computed on the host), P < 1 or NULL alphas /
+ * betas CTCDEC_E_INVALID. */
+int ctcdec_decode_batch_lm_sweep_async(const ctcdec_config *cfg, void *scorer, const void *input, int dtype,
+                                       const int32_t *seq_lens, int B, int T, const double *alphas,
+                                       const double *betas, int P, int32_t *tokens, int32_t *timesteps, float *scores,
+                                       int32_t *lens, int32_t *n_results, int32_t *flags, float *log_probs_out,
+                                       void *workspace, size_t workspace_bytes, void *stream);
+
 /* ---- streaming (OnlineCTCBeamDecoder) ------------------------------------------------------------- */
 
 /* Replaces: paddle_get_decoder_state (binding.cpp:246-261).  The state (beam + trie + absolute frame
