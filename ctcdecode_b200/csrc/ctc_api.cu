@@ -212,24 +212,34 @@ static int make_plan(const ctcdec_config *cfg, int B, int T, Plan *pl, bool lm =
   return CTCDEC_OK;
 }
 
-template <int NT, bool SORTED, bool LM, int KPT, bool TIMING>
-static int launch_beam_k(const BeamParams &bp, int B, cudaStream_t s) {
-  // raise the dynamic shared-memory limit once per device and size: cudaFuncSetAttribute on a kernel that is
-  // running waits for it, which would serialise the utterance groups the host entry point pipelines
+// Raises kernel Kern's dynamic shared-memory limit on the current device to `bytes`, once per device and size:
+// cudaFuncSetAttribute on a kernel that is running waits for it, which would serialise the utterance groups the host
+// entry point pipelines.  A limit that is not raised yet is refused while a stream is being captured.  (Keyed on the
+// kernel itself: every beam_kernel instance has the same function type.)
+template <auto Kern>
+static int raise_smem_limit(size_t bytes, const char *what) {
+  if (bytes <= 48 * 1024) return CTCDEC_OK;
   static std::atomic<int> limit[64];
   static std::mutex limit_mu;
   int dev = 0;
   CU(cudaGetDevice(&dev));
-  const int smem_bytes = bp.L.total + (TIMING ? 4096 : 0);  // TIMING: [16][32] per-warp counters behind the layout
-  if (smem_bytes > limit[dev & 63].load(std::memory_order_acquire)) {
-    if (g_capturing) return fail(CTCDEC_E_UNSUPPORTED, "beam kernel not prepared on device %d: %s", dev, kCaptureFirst);
+  if ((int)bytes > limit[dev & 63].load(std::memory_order_acquire)) {
+    if (g_capturing) return fail(CTCDEC_E_UNSUPPORTED, "%s kernel not prepared on device %d: %s", what, dev, kCaptureFirst);
     std::lock_guard<std::mutex> lk(limit_mu);  // (check again under the lock: two host threads, same device)
-    if (smem_bytes > limit[dev & 63].load(std::memory_order_acquire)) {
-      CU(cudaFuncSetAttribute(beam_kernel<NT, SORTED, LM, KPT, TIMING>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes));
-      limit[dev & 63].store(smem_bytes, std::memory_order_release);
+    if ((int)bytes > limit[dev & 63].load(std::memory_order_acquire)) {
+      CU(cudaFuncSetAttribute(Kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+      limit[dev & 63].store((int)bytes, std::memory_order_release);
     }
   }
-  beam_kernel<NT, SORTED, LM, KPT, TIMING><<<B, NT, bp.L.total + (TIMING ? 4096 : 0), s>>>(bp);
+  return CTCDEC_OK;
+}
+
+template <int NT, bool SORTED, bool LM, int KPT, bool TIMING>
+static int launch_beam_k(const BeamParams &bp, int B, cudaStream_t s) {
+  const int smem_bytes = bp.L.total + (TIMING ? 4096 : 0);  // TIMING: [16][32] per-warp counters behind the layout
+  int rc = raise_smem_limit<beam_kernel<NT, SORTED, LM, KPT, TIMING>>(smem_bytes, "beam");
+  if (rc) return rc;
+  beam_kernel<NT, SORTED, LM, KPT, TIMING><<<B, NT, smem_bytes, s>>>(bp);
   CU(cudaGetLastError());
   return CTCDEC_OK;
 }
@@ -298,26 +308,17 @@ struct PruneInput {
 
 template <bool SORTED, int KPL, bool LOGITS>
 static int launch_prune_k(const PruneParams &pp, int grid, int threads, size_t smem, cudaStream_t s) {
-  if (smem > 48 * 1024) {
-    static std::atomic<int> limit[64];
-    static std::mutex limit_mu;
-    int dev = 0;
-    CU(cudaGetDevice(&dev));
-    if ((int)smem > limit[dev & 63].load(std::memory_order_acquire)) {
-      if (g_capturing) return fail(CTCDEC_E_UNSUPPORTED, "prune kernel not prepared on device %d: %s", dev, kCaptureFirst);
-      std::lock_guard<std::mutex> lk(limit_mu);
-      if ((int)smem > limit[dev & 63].load(std::memory_order_acquire)) {
-        CU(cudaFuncSetAttribute(prune_kernel<SORTED, KPL, LOGITS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        limit[dev & 63].store((int)smem, std::memory_order_release);
-      }
-    }
-  }
+  const int rc = raise_smem_limit<prune_kernel<SORTED, KPL, LOGITS>>(smem, "prune");
+  if (rc) return rc;
   prune_kernel<SORTED, KPL, LOGITS><<<grid, threads, smem, s>>>(pp);
   return CTCDEC_OK;
 }
 
+// the prune scan of B utterances into the pruned rows and characters of the plan's workspace ws
 static int launch_prune(const ctcdec_config *cfg, const Plan &pl, const PruneInput &in, const int *seq_lens, int B,
-                        int T, float *lp, uint16_t *idx, int *flags, cudaStream_t s) {
+                        int T, unsigned char *ws, int *flags, cudaStream_t s) {
+  float *const lp = reinterpret_cast<float *>(ws + pl.off_lp);
+  uint16_t *const idx = pl.sorted ? reinterpret_cast<uint16_t *>(ws + pl.off_idx) : nullptr;
   PruneParams pp;
   memset(&pp, 0, sizeof(pp));
   const bool logits = in.kind != IN_F32;
@@ -361,20 +362,8 @@ static int launch_prune(const ctcdec_config *cfg, const Plan &pl, const PruneInp
 
 static int launch_finalize(const BeamParams &bp, int B, cudaStream_t s) {
   const size_t smem = finalize_smem_bytes(bp.K);
-  if (smem > 48 * 1024) {
-    static std::atomic<int> limit[64];
-    static std::mutex limit_mu;
-    int dev = 0;
-    CU(cudaGetDevice(&dev));
-    if ((int)smem > limit[dev & 63].load(std::memory_order_acquire)) {
-      if (g_capturing) return fail(CTCDEC_E_UNSUPPORTED, "finalize kernel not prepared on device %d: %s", dev, kCaptureFirst);
-      std::lock_guard<std::mutex> lk(limit_mu);
-      if ((int)smem > limit[dev & 63].load(std::memory_order_acquire)) {
-        CU(cudaFuncSetAttribute(finalize_kernel<1024>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        limit[dev & 63].store((int)smem, std::memory_order_release);
-      }
-    }
-  }
+  const int rc = raise_smem_limit<finalize_kernel<1024>>(smem, "finalize");
+  if (rc) return rc;
   // 1024 threads: the backtrace is a latency-bound pointer chase, its only resource is chains in flight
   finalize_kernel<1024><<<B, 1024, smem, s>>>(bp);
   CU(cudaGetLastError());
@@ -396,17 +385,55 @@ static int check_device() {
   return CTCDEC_OK;
 }
 
+// makes `device` (an index of the per-device cache and locks) the current device and checks it
+static int use_device(int device) {
+  if (device < 0 || device >= 64) return fail(CTCDEC_E_INVALID, "device %d out of range", device);
+  if (cudaSetDevice(device) != cudaSuccess)
+    return fail(CTCDEC_E_NO_DEVICE, "cudaSetDevice(%d) failed (this library has no CPU fallback)", device);
+  return check_device();
+}
+
+// the current device, checked, for the entry points that run on the caller's device and use its cache or lock
+static int current_device(int *device) {
+  const int rc = check_device();
+  if (rc) return rc;
+  CU(cudaGetDevice(device));
+  if (*device >= 64) return fail(CTCDEC_E_INVALID, "device %d out of range", *device);
+  return CTCDEC_OK;
+}
+
+// dtype -1 (probabilities, where the entry point takes them) or a CTCDEC_DTYPE_* of logits -> the prune input kind
+static int input_kind(int dtype, bool probs, int *kind) {
+  if ((dtype != -1 || !probs) && dtype != CTCDEC_DTYPE_F32 && dtype != CTCDEC_DTYPE_F16 && dtype != CTCDEC_DTYPE_BF16)
+    return probs ? fail(CTCDEC_E_INVALID, "dtype %d is not -1 (probabilities) or one of CTCDEC_DTYPE_F32 / F16 / BF16", dtype)
+                 : fail(CTCDEC_E_INVALID, "dtype %d is not one of CTCDEC_DTYPE_F32 / F16 / BF16", dtype);
+  *kind = dtype == -1 ? IN_F32 : dtype == CTCDEC_DTYPE_F32 ? IN_LOGITS_F32
+        : dtype == CTCDEC_DTYPE_F16 ? IN_LOGITS_F16 : IN_LOGITS_BF16;
+  return CTCDEC_OK;
+}
+
+// the 256-byte aligned start of a workspace; the sizes the library asks for include the 256 bytes this may skip
+static unsigned char *align256(void *p) {
+  return reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(p) + 255) / 256 * 256);
+}
+
 // ---------------------------------------------------------------------------------------------------
 //  per-device cache for the host-buffer entry points (stream + grow-only device buffers)
 // ---------------------------------------------------------------------------------------------------
 constexpr int kHostChunks = 8;  // utterance groups (streams) the host-buffer entry point pipelines over
+// device buffers: the input rows, the seq_lens of ctcdec_decode_batch_host, the token / timestep rows, the small
+// outputs (small_out), the workspace, the per-call tables of a streaming chunk
+enum CacheSlot { kBufInput, kBufSeqLens, kBufTokens, kBufTimesteps, kBufSmall, kBufWork, kBufStreamTab, kBufSlots };
+// pinned host memory: the hook scorer's exchange blocks (new-node lists, LM updates, abort flag), the small outputs,
+// the staged token / timestep rows
+enum PinSlot { kPinNewList, kPinUpdates, kPinAbort, kPinSmall, kPinRows, kPinSlots };
 struct DevCache {
   cudaStream_t stream = nullptr;
   cudaStream_t cs[kHostChunks] = {};
-  void *buf[12] = {};
-  size_t cap[12] = {};
-  void *pin[6] = {};  // pinned host staging (scorer path: new-node lists, LM updates; [4]: n_results / flags)
-  size_t pcap[6] = {};
+  void *buf[kBufSlots] = {};
+  size_t cap[kBufSlots] = {};
+  void *pin[kPinSlots] = {};
+  size_t pcap[kPinSlots] = {};
   cudaEvent_t beam_ev = nullptr;  // scorer path: recorded just before the persistent beam launch
 };
 static DevCache g_cache[64];
@@ -470,6 +497,71 @@ static void spread_rows(const int *stage_tok, const int *stage_ts, int32_t *toke
   for (unsigned w = 1; w < nt; ++w) pool.emplace_back(work, w);
   work(0);
   for (auto &th : pool) th.join();
+}
+
+// rows of `bytes` go through the staging when the caller's arrays are pageable and the staging stays small enough
+static bool stage_rows(const void *tokens, const void *timesteps, size_t bytes) {
+  return bytes <= kMaxRowStaging && !(host_ptr_is_pinned(tokens) && host_ptr_is_pinned(timesteps));
+}
+
+// Enqueues columns [0, max_len) of `rows` token / timestep rows of row_stride columns from the device: compactly into
+// the staging ([rows][max_len] each, for spread_rows once s has finished) if stage_tok is given, else by DMA into the
+// caller's arrays.
+static int enqueue_rows(const int32_t *d_tok, const int32_t *d_ts, int32_t *tokens, int32_t *timesteps,
+                        int32_t *stage_tok, int32_t *stage_ts, size_t rows, int max_len, int row_stride, cudaStream_t s) {
+  const size_t src_pitch = (size_t)row_stride * 4, pitch = (size_t)(stage_tok ? max_len : row_stride) * 4;
+  CU(cudaMemcpy2DAsync(stage_tok ? stage_tok : tokens, pitch, d_tok, src_pitch, (size_t)max_len * 4, rows,
+                       cudaMemcpyDeviceToHost, s));
+  CU(cudaMemcpy2DAsync(stage_ts ? stage_ts : timesteps, pitch, d_ts, src_pitch, (size_t)max_len * 4, rows,
+                       cudaMemcpyDeviceToHost, s));
+  return CTCDEC_OK;
+}
+
+// The [B, K] scores and lens and the [B] n_results and flags of a decode.  In the cache (slot kBufSmall, and its pinned
+// staging kPinSmall) they share one block, laid out by small_out, with flags = n_results + B.
+struct SmallOut { float *scores; int32_t *lens, *n_results, *flags; };
+static size_t small_bytes(int B, int K) { return (size_t)B * K * 4 * 2 + (size_t)B * 8 + 1024; }
+static SmallOut small_out(void *p, int B, int K) {
+  const size_t n_bk = (size_t)B * K;
+  SmallOut o;
+  o.scores = static_cast<float *>(p);
+  o.lens = reinterpret_cast<int32_t *>(static_cast<char *>(p) + al256(n_bk * 4));
+  o.n_results = reinterpret_cast<int32_t *>(static_cast<char *>(p) + 2 * al256(n_bk * 4));
+  o.flags = o.n_results + B;
+  return o;
+}
+
+// Enqueues the copy of utterances [b0, b0 + nb) of the small outputs d into the pinned staging h (pinned: a copy into
+// pageable memory would block the calling thread until the work before it has finished).
+static int read_small(const SmallOut &h, const SmallOut &d, int K, int b0, int nb, cudaStream_t s) {
+  const size_t ko = (size_t)b0 * K, bytes = (size_t)nb * K * 4;
+  CU(cudaMemcpyAsync(h.scores + ko, d.scores + ko, bytes, cudaMemcpyDeviceToHost, s));
+  CU(cudaMemcpyAsync(h.lens + ko, d.lens + ko, bytes, cudaMemcpyDeviceToHost, s));
+  CU(cudaMemcpyAsync(h.n_results + b0, d.n_results + b0, (size_t)nb * 4, cudaMemcpyDeviceToHost, s));
+  CU(cudaMemcpyAsync(h.flags + b0, d.flags + b0, (size_t)nb * 4, cudaMemcpyDeviceToHost, s));
+  return CTCDEC_OK;
+}
+
+// Rows p < n_results[b] of the staged scores and lens into the caller's [B, K] arrays, for the utterances in `mask`
+// (all if NULL).  The other rows stay as the caller left them: the finalize kernel does not write them, and the device
+// buffers are reused between calls (reference binding.cpp:79-99 writes results.size() rows).
+static void copy_result_rows(const SmallOut &h, int B, int K, const uint8_t *mask, float *scores, int32_t *lens) {
+  for (int b = 0; b < B; ++b) {
+    if (mask && !mask[b]) continue;
+    const size_t nr = (size_t)std::max(0, std::min(h.n_results[b], K));
+    memcpy(scores + (size_t)b * K, h.scores + (size_t)b * K, nr * 4);
+    memcpy(lens + (size_t)b * K, h.lens + (size_t)b * K, nr * 4);
+  }
+}
+
+// The longest result of utterances [b0, b0 + nb) (those in `mask`, if given).  Only rows p < n_results[b] count: the
+// lens of the others are whatever the caller's arrays held (the reference's Python zero-fills out_seq_len).
+static int max_result_len(const SmallOut &h, int K, int b0, int nb, const uint8_t *mask) {
+  int max_len = 0;
+  for (int b = b0; b < b0 + nb; ++b)
+    if (!mask || mask[b])
+      for (int p = 0; p < h.n_results[b] && p < K; ++p) max_len = std::max(max_len, h.lens[(size_t)b * K + p]);
+  return max_len;
 }
 
 // completion of device-path work (ctcdec_decode_stream_device / ctcdec_stream_committed_device) on a state; one event
@@ -657,6 +749,112 @@ static int serve_handshakes(HostScorer *sc, int B, int K, const int *need, TrieM
   return failed.load();
 }
 
+// the caller's outputs of a decode (device memory)
+struct DecodeOut {
+  int32_t *tokens, *timesteps;  // [B, K, out_T]
+  float *scores;                // [B, K]
+  int32_t *lens;                // [B, K]
+  int32_t *n_results, *flags;   // [B]
+};
+
+// The kernel parameters every decode shares: the pruned rows in the plan's workspace ws, the outputs and the knobs.
+// The caller adds the arenas and states (one flat region, or the per-stream tables), tile_frames, fresh and a scorer.
+static BeamParams beam_params(const ctcdec_config &cfg, const Plan &pl, const unsigned char *ws, const int *seq_lens,
+                              int T, const DecodeOut &o, int out_T) {
+  BeamParams bp;
+  memset(&bp, 0, sizeof(bp));
+  bp.lp = reinterpret_cast<const float *>(ws + pl.off_lp);
+  bp.idx = pl.sorted ? reinterpret_cast<const uint16_t *>(ws + pl.off_idx) : nullptr;
+  bp.seq_lens = seq_lens; bp.T = T; bp.V = cfg.vocab_size; bp.NP = pl.NP; bp.K = cfg.beam_size; bp.blank = cfg.blank_id;
+  bp.out_tokens = o.tokens; bp.out_timesteps = o.timesteps; bp.out_scores = o.scores; bp.out_lens = o.lens;
+  bp.n_results = o.n_results; bp.out_T = out_T; bp.flags = o.flags;
+  bp.timing = g_prof.timing;
+  bp.force_fallback = getenv("CTCDEC_FORCE_FALLBACK") ? 1 : 0;  // test knob
+  return bp;
+}
+
+// the flat arenas and states of an offline decode, in the plan's workspace ws
+static void flat_arenas(BeamParams &bp, const Plan &pl, unsigned char *ws) {
+  bp.arena = reinterpret_cast<Node *>(ws + pl.off_arena); bp.arena_stride = pl.arena_stride;
+  bp.state = reinterpret_cast<int *>(ws + pl.off_state); bp.state_stride = pl.state_stride;
+  bp.arena_cap = (int)pl.arena_stride;
+}
+
+// The scorer's part of the kernel parameters (its dictionary must be on the device): the dictionary and the word
+// bonus, and for an n-gram scorer, whose tables must be on the device too, the model the beam kernel scores with.
+static void attach_scorer(BeamParams &bp, const HostScorer &sc) {
+  bp.dict_next = sc.d_next; bp.dict_mask = sc.d_mask; bp.dict_wc = sc.dict.wc; bp.dict_start = sc.dict.start;
+  bp.space_id = sc.space_id; bp.beta = sc.beta; bp.lm_char = sc.is_character_based ? 1 : 0;
+  if (sc.ngram) {
+    bp.lm_dev = 1; bp.lm_alpha = sc.alpha; bp.ngram = sc.d_view;
+    bp.word_of_state = sc.d_word_of_state; bp.label_word = sc.d_label_word; bp.lm_hist_n = sc.max_order - 1;
+  }
+}
+
+// The pinned exchange blocks of a hook scorer's handshake (beam_core.cuh) for B utterances, in the cache c, and the
+// kernel parameters that point at them: headers cleared, abort flag down, and for a character-based model the root's
+// row of LM terms in the update block of each utterance in `at_root` (all if NULL), the first entry its CTA picks up.
+static int prepare_exchange(DevCache &c, HostScorer &sc, int B, const uint8_t *at_root, BeamParams &bp) {
+  int nls = 0, ups = 0;
+  exchange_strides(bp.K, exchange_row_len(sc), &nls, &ups);
+  int rc = ensure_pinned(c, kPinNewList, (size_t)B * nls * 4);
+  if (rc || (rc = ensure_pinned(c, kPinUpdates, (size_t)B * ups * 4)) || (rc = ensure_pinned(c, kPinAbort, 256))) return rc;
+  int *h_newlist = (int *)c.pin[kPinNewList], *h_upd = (int *)c.pin[kPinUpdates];
+  for (int b = 0; b < B; ++b) { memset(h_newlist + (size_t)b * nls, 0, 16); memset(h_upd + (size_t)b * ups, 0, 8); }
+  if (sc.is_character_based) {  // (computed once, copied to the others)
+    const int *root = nullptr;
+    std::vector<int> scratch;
+    for (int b = 0; b < B; ++b) {
+      if (at_root && !at_root[b]) continue;
+      int *up = h_upd + (size_t)b * ups;
+      if (root) memcpy(up, root, (size_t)(3 + bp.V) * 4);
+      else { lm_char_root_entry(sc, sc.cond_caches[0], up, scratch); root = up; }
+    }
+  }
+  *static_cast<int *>(c.pin[kPinAbort]) = 0;
+  // The per-frame exchange with the host goes through pinned, device-mapped host memory (unified addressing): the
+  // kernel reads the few LM updates and writes the new-node list straight over PCIe, with no memcpy calls.
+  bp.newlist = h_newlist; bp.lm_upd = h_upd; bp.lm_nl_stride = nls; bp.lm_up_stride = ups;
+  return CTCDEC_OK;
+}
+
+// One persistent launch of the beam kernel with a hook scorer (after prepare_exchange), served by serve_handshakes until
+// utterance b has been answered answers[b] frames, and synchronised.  After each frame a CTA publishes its new nodes in
+// mapped host memory, raises its done flag and polls its go flag; CTAs never wait on each other, so the scheme needs no
+// co-residency, and a kernel-side deadline and the abort flag bound every wait.  `what` names the path in errors.
+static int run_handshake(const BeamParams &bp_in, const Plan &pl, int B, HostScorer *sc, DevCache &c, const int *answers,
+                         TrieMirror *const *mirrors, HandshakeStats *stats, const char *what, cudaStream_t s) {
+  BeamParams bp = bp_in;
+  auto *const hs_abort = static_cast<std::atomic<int> *>(c.pin[kPinAbort]);
+  bp.lm_persistent = 1; bp.hs_abort = static_cast<int *>(c.pin[kPinAbort]);
+  if (!c.beam_ev) CU(cudaEventCreateWithFlags(&c.beam_ev, cudaEventDisableTiming));
+  CU(cudaEventRecord(c.beam_ev, s));
+  const int rc = launch_beam(bp, pl, B, s);
+  if (rc) return rc;
+  // the handshake gives up after 8 s without progress: start its clock once the work queued on s before the beam
+  // kernel (the caller's, on a stream of the caller's) has finished
+  const cudaError_t ew = cudaEventSynchronize(c.beam_ev);
+  if (ew != cudaSuccess) {
+    hs_abort->store(1, std::memory_order_release);
+    return fail(CTCDEC_E_CUDA, "work queued before the beam kernel (%s): %s", what, cudaGetErrorString(ew));
+  }
+  const int failed = serve_handshakes(sc, B, bp.K, answers, mirrors, (int *)c.pin[kPinNewList],
+                                      (int *)c.pin[kPinUpdates], stats);
+  if (failed) hs_abort->store(1, std::memory_order_release);
+  const cudaError_t e = cudaStreamSynchronize(s);
+  if (e != cudaSuccess) return fail(CTCDEC_E_CUDA, "beam kernel (%s): %s", what, cudaGetErrorString(e));
+  if (failed) return fail(CTCDEC_E_CUDA, "beam kernel (%s) stopped answering the per-frame handshake", what);
+  return CTCDEC_OK;
+}
+
+// the caller's workspace, 256-byte aligned, which must hold `need` bytes (need includes the 256 the alignment may skip)
+static int workspace_start(void *workspace, size_t workspace_bytes, size_t need, unsigned char **ws) {
+  if (!workspace || workspace_bytes < need)
+    return fail(CTCDEC_E_WORKSPACE, "workspace of %zu bytes given, %zu needed", workspace_bytes, need);
+  *ws = align256(workspace);
+  return CTCDEC_OK;
+}
+
 }  // namespace ctc
 
 using namespace ctc;
@@ -695,22 +893,12 @@ static int decode_device_impl(const ctcdec_config *cfg, const PruneInput &in, co
   if (B == 0) return CTCDEC_OK;
   if (!in.data && T > 0) return fail(CTCDEC_E_INVALID, "probs is NULL");
   if (!tokens || !timesteps || !scores || !lens) return fail(CTCDEC_E_INVALID, "an output pointer is NULL");
-  unsigned char *ws = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(workspace) + 255) / 256 * 256);
-  if (!workspace || ws + pl.total > reinterpret_cast<unsigned char *>(workspace) + workspace_bytes)
-    return fail(CTCDEC_E_WORKSPACE, "workspace of %zu bytes given, %zu needed", workspace_bytes, pl.total + 256);
+  unsigned char *ws = nullptr;
+  if ((rc = workspace_start(workspace, workspace_bytes, pl.total + 256, &ws))) return rc;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-  // n_results / flags are optional for the caller: park them at the end of the state area if absent
-  int *state = reinterpret_cast<int *>(ws + pl.off_state);
-  // flags are OR-accumulated by the prune and finalize kernels
-  int *flags_dev = flags;
-  int *nres_dev = n_results;
-  // (state_stride is padded to >= 64 ints beyond need only when K is tiny; keep explicit scratch instead)
-  static_assert(kStateHeader == 4, "state header");
-  if (!flags_dev || !nres_dev) return fail(CTCDEC_E_INVALID, "n_results and flags device buffers are required by the device entry point");
-  CU(cudaMemsetAsync(flags_dev, 0, (size_t)B * 4, s));
+  if (!flags || !n_results) return fail(CTCDEC_E_INVALID, "n_results and flags device buffers are required by the device entry point");
+  CU(cudaMemsetAsync(flags, 0, (size_t)B * 4, s));  // (OR-accumulated by the prune and finalize kernels)
 
-  float *lp = reinterpret_cast<float *>(ws + pl.off_lp);
-  uint16_t *idx = pl.sorted ? reinterpret_cast<uint16_t *>(ws + pl.off_idx) : nullptr;
   const bool prof = g_prof.on;
   if (prof) {
     for (int i = 0; i < 4; ++i)
@@ -718,19 +906,12 @@ static int decode_device_impl(const ctcdec_config *cfg, const PruneInput &in, co
     g_prof.valid = false;
     CU(cudaEventRecord(g_prof.ev[0], s));
   }
-  if ((rc = launch_prune(cfg, pl, in, seq_lens, B, T, lp, idx, flags_dev, s))) return rc;
+  if ((rc = launch_prune(cfg, pl, in, seq_lens, B, T, ws, flags, s))) return rc;
   if (prof) CU(cudaEventRecord(g_prof.ev[1], s));
 
-  BeamParams bp;
-  memset(&bp, 0, sizeof(bp));
-  bp.lp = lp; bp.idx = idx; bp.seq_lens = seq_lens; bp.T = T; bp.V = cfg->vocab_size; bp.NP = pl.NP;
-  bp.K = cfg->beam_size; bp.blank = cfg->blank_id; bp.tile_frames = pl.F;
-  bp.arena = reinterpret_cast<Node *>(ws + pl.off_arena); bp.arena_stride = pl.arena_stride;
-  bp.state = state; bp.state_stride = pl.state_stride; bp.arena_cap = (int)pl.arena_stride; bp.fresh = 1;
-  bp.out_tokens = tokens; bp.out_timesteps = timesteps; bp.out_scores = scores; bp.out_lens = lens;
-  bp.n_results = nres_dev; bp.out_T = T; bp.flags = flags_dev;
-  bp.timing = g_prof.timing;
-  bp.force_fallback = getenv("CTCDEC_FORCE_FALLBACK") ? 1 : 0;  // test knob
+  BeamParams bp = beam_params(*cfg, pl, ws, seq_lens, T, DecodeOut{tokens, timesteps, scores, lens, n_results, flags}, T);
+  flat_arenas(bp, pl, ws);
+  bp.tile_frames = pl.F; bp.fresh = 1;
   if ((rc = launch_beam(bp, pl, B, s))) return rc;
   if (prof) CU(cudaEventRecord(g_prof.ev[2], s));
   if ((rc = launch_finalize(bp, B, s))) return rc;
@@ -753,9 +934,9 @@ int ctcdec_decode_batch_device_logits(const ctcdec_config *cfg, const void *logi
                                       int B, int T, int32_t *tokens, int32_t *timesteps, float *scores, int32_t *lens,
                                       int32_t *n_results, int32_t *flags, float *log_probs_out, void *workspace,
                                       size_t workspace_bytes, void *stream) {
-  if (dtype != CTCDEC_DTYPE_F32 && dtype != CTCDEC_DTYPE_F16 && dtype != CTCDEC_DTYPE_BF16)
-    return fail(CTCDEC_E_INVALID, "dtype %d is not one of CTCDEC_DTYPE_F32 / F16 / BF16", dtype);
-  const int kind = dtype == CTCDEC_DTYPE_F32 ? IN_LOGITS_F32 : dtype == CTCDEC_DTYPE_F16 ? IN_LOGITS_F16 : IN_LOGITS_BF16;
+  int kind = 0;
+  const int rc = input_kind(dtype, false, &kind);
+  if (rc) return rc;
   return decode_device_impl(cfg, PruneInput{logits, kind, log_probs_out}, seq_lens, B, T, tokens, timesteps, scores,
                             lens, n_results, flags, workspace, workspace_bytes, stream);
 }
@@ -807,10 +988,7 @@ int ctcdec_decode_batch_host(const ctcdec_config *cfg, const float *probs, const
                              int32_t *flags, int device) {
   Plan pl;
   int rc = make_plan(cfg, B, T, &pl);
-  if (rc) return rc;
-  if (device < 0 || device >= 64) return fail(CTCDEC_E_INVALID, "device %d out of range", device);
-  if (cudaSetDevice(device) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "cudaSetDevice(%d) failed (this library has no CPU fallback)", device);
-  if ((rc = check_device())) return rc;
+  if (rc || (rc = use_device(device))) return rc;
   if (B == 0) return CTCDEC_OK;
   std::lock_guard<std::mutex> lock(g_mu[device]);
   DevCache &c = g_cache[device];
@@ -829,29 +1007,21 @@ int ctcdec_decode_batch_host(const ctcdec_config *cfg, const float *probs, const
   Plan plc;
   if ((rc = make_plan(cfg, chunk, T, &plc))) return rc;
   const size_t ws_stride = al256(plc.total + 512);
-  const size_t n_probs = (size_t)B * T * V, n_out = (size_t)B * K * T, n_bk = (size_t)B * K;
-  if ((rc = ensure(c, 0, n_probs * 4 + 256))) return rc;
-  if ((rc = ensure(c, 1, (size_t)B * 4 + 256))) return rc;
-  if ((rc = ensure(c, 2, n_out * 4 + 256))) return rc;
-  if ((rc = ensure(c, 3, n_out * 4 + 256))) return rc;
-  if ((rc = ensure(c, 4, n_bk * 4 * 2 + (size_t)B * 8 + 1024))) return rc;
-  if ((rc = ensure(c, 5, ws_stride * C))) return rc;
-  float *d_probs = (float *)c.buf[0];
-  int *d_lens_in = seq_lens ? (int *)c.buf[1] : nullptr;
-  int *d_tok = (int *)c.buf[2], *d_ts = (int *)c.buf[3];
-  float *d_scores = (float *)c.buf[4];
-  int *d_lens = (int *)((char *)c.buf[4] + al256(n_bk * 4));
-  int *d_nres = (int *)((char *)d_lens + al256(n_bk * 4));
-  int *d_flags = d_nres + B;
-  // (pinned: a device-to-host copy into pageable memory would block this thread until the group has finished)
-  if ((rc = ensure_pinned(c, 4, (size_t)B * 8 + n_bk * 8))) return rc;
-  int *const h_nres = static_cast<int *>(c.pin[4]);
-  int *const h_flags = h_nres + B;
-  float *const h_scores = reinterpret_cast<float *>(h_flags + B);
-  int *const h_lens = reinterpret_cast<int *>(h_scores + n_bk);
-  const bool staged = n_out > 0 && n_out * 8 <= kMaxRowStaging && !(host_ptr_is_pinned(tokens) && host_ptr_is_pinned(timesteps));
-  if (staged && (rc = ensure_pinned(c, 5, n_out * 8))) return rc;
-  int *const stage_tok = staged ? static_cast<int *>(c.pin[5]) : nullptr;
+  const size_t n_probs = (size_t)B * T * V, n_out = (size_t)B * K * T;
+  if ((rc = ensure(c, kBufInput, n_probs * 4 + 256))) return rc;
+  if ((rc = ensure(c, kBufSeqLens, (size_t)B * 4 + 256))) return rc;
+  if ((rc = ensure(c, kBufTokens, n_out * 4 + 256))) return rc;
+  if ((rc = ensure(c, kBufTimesteps, n_out * 4 + 256))) return rc;
+  if ((rc = ensure(c, kBufSmall, small_bytes(B, K)))) return rc;
+  if ((rc = ensure(c, kBufWork, ws_stride * C))) return rc;
+  if ((rc = ensure_pinned(c, kPinSmall, small_bytes(B, K)))) return rc;
+  float *d_probs = (float *)c.buf[kBufInput];
+  int *d_lens_in = seq_lens ? (int *)c.buf[kBufSeqLens] : nullptr;
+  int *d_tok = (int *)c.buf[kBufTokens], *d_ts = (int *)c.buf[kBufTimesteps];
+  const SmallOut d = small_out(c.buf[kBufSmall], B, K), h = small_out(c.pin[kPinSmall], B, K);
+  const bool staged = n_out > 0 && stage_rows(tokens, timesteps, n_out * 8);
+  if (staged && (rc = ensure_pinned(c, kPinRows, n_out * 8))) return rc;
+  int *const stage_tok = staged ? static_cast<int *>(c.pin[kPinRows]) : nullptr;
   int *const stage_ts = staged ? stage_tok + n_out : nullptr;
   int chunk_len[kHostChunks] = {};
   for (int i = 0; i < C; ++i) {
@@ -861,44 +1031,23 @@ int ctcdec_decode_batch_host(const ctcdec_config *cfg, const float *probs, const
     if (n_probs) CU(cudaMemcpyAsync(d_probs + po, probs + po, (size_t)nb * T * V * 4, cudaMemcpyHostToDevice, s));
     if (seq_lens) CU(cudaMemcpyAsync(d_lens_in + b0, seq_lens + b0, (size_t)nb * 4, cudaMemcpyHostToDevice, s));
     rc = ctcdec_decode_batch_device(cfg, d_probs + po, seq_lens ? d_lens_in + b0 : nullptr, nb, T, d_tok + oo, d_ts + oo,
-                                    d_scores + ko, d_lens + ko, d_nres + b0, d_flags + b0,
-                                    (char *)c.buf[5] + ws_stride * i, ws_stride, s);
-    if (rc) return rc;
+                                    d.scores + ko, d.lens + ko, d.n_results + b0, d.flags + b0,
+                                    (char *)c.buf[kBufWork] + ws_stride * i, ws_stride, s);
     // small results first: lens tell how many columns of the big tensors carry data
-    CU(cudaMemcpyAsync(h_scores + ko, d_scores + ko, (size_t)nb * K * 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(h_lens + ko, d_lens + ko, (size_t)nb * K * 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(h_nres + b0, d_nres + b0, (size_t)nb * 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(h_flags + b0, d_flags + b0, (size_t)nb * 4, cudaMemcpyDeviceToHost, s));
+    if (rc || (rc = read_small(h, d, K, b0, nb, s))) return rc;
   }
   for (int i = 0; i < C; ++i) {
     const int b0 = i * chunk, nb = std::min(chunk, B - b0);
     cudaStream_t s = c.cs[i];
     CU(cudaStreamSynchronize(s));
-    // The reference leaves rows p >= n_results and columns >= len untouched; lens of untouched rows are
-    // whatever the caller put there (the reference's Python zero-fills out_seq_len), so only trust rows
-    // below n_results when sizing the column window.
-    int max_len = 0;
-    for (int b = b0; b < b0 + nb; ++b) {
-      const int nr = h_nres[b];
-      for (int p = 0; p < nr && p < K; ++p) max_len = std::max(max_len, h_lens[(size_t)b * K + p]);
-    }
-    if (max_len > T) max_len = T;
-    chunk_len[i] = max_len;
-    if (max_len > 0) {
-      const size_t oo = (size_t)b0 * K * T;
-      int32_t *const dt = staged ? stage_tok + oo : tokens + oo, *const ds = staged ? stage_ts + oo : timesteps + oo;
-      const size_t pitch = (size_t)(staged ? max_len : T) * 4;
-      CU(cudaMemcpy2DAsync(dt, pitch, d_tok + oo, (size_t)T * 4, (size_t)max_len * 4, (size_t)nb * K, cudaMemcpyDeviceToHost, s));
-      CU(cudaMemcpy2DAsync(ds, pitch, d_ts + oo, (size_t)T * 4, (size_t)max_len * 4, (size_t)nb * K, cudaMemcpyDeviceToHost, s));
-    }
+    chunk_len[i] = std::min(max_result_len(h, K, b0, nb, nullptr), T);
+    const size_t oo = (size_t)b0 * K * T;
+    if (chunk_len[i] > 0 && (rc = enqueue_rows(d_tok + oo, d_ts + oo, tokens + oo, timesteps + oo,
+                                               staged ? stage_tok + oo : nullptr, staged ? stage_ts + oo : nullptr,
+                                               (size_t)nb * K, chunk_len[i], T, s)))
+      return rc;
   }
-  // rows p >= n_results[b] stay as the caller left them (the finalize kernel does not write them, and the
-  // device buffers are reused between calls; reference: binding.cpp:79-99 writes results.size() rows)
-  for (int b = 0; b < B; ++b) {
-    const size_t nr = (size_t)std::max(0, std::min(h_nres[b], K));
-    memcpy(scores + (size_t)b * K, h_scores + (size_t)b * K, nr * 4);
-    memcpy(lens + (size_t)b * K, h_lens + (size_t)b * K, nr * 4);
-  }
+  copy_result_rows(h, B, K, nullptr, scores, lens);
   for (int i = 0; i < C; ++i) {
     CU(cudaStreamSynchronize(c.cs[i]));
     if (staged && chunk_len[i] > 0) {  // (the later groups' rows are still on their way meanwhile)
@@ -907,9 +1056,9 @@ int ctcdec_decode_batch_host(const ctcdec_config *cfg, const float *probs, const
       spread_rows(stage_tok + oo, stage_ts + oo, tokens + oo, timesteps + oo, (size_t)nb * K, chunk_len[i], T);
     }
   }
-  if (n_results) memcpy(n_results, h_nres, (size_t)B * 4);
-  if (flags) memcpy(flags, h_flags, (size_t)B * 4);
-  return check_error_flags(h_flags, B);
+  if (n_results) memcpy(n_results, h.n_results, (size_t)B * 4);
+  if (flags) memcpy(flags, h.flags, (size_t)B * 4);
+  return check_error_flags(h.flags, B);
 }
 
 int ctcdec_decode_batch_host_multi(const ctcdec_config *cfg, const float *probs, const int32_t *seq_lens, int B, int T,
@@ -993,8 +1142,7 @@ static int state_create(const ctcdec_config *cfg, int device, bool lm, void **st
   int rc = make_plan(cfg, 1, 1, &pl, lm);
   if (rc) return rc;
   if (!state) return fail(CTCDEC_E_INVALID, "state is NULL");
-  if (cudaSetDevice(device) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "cudaSetDevice(%d) failed (this library has no CPU fallback)", device);
-  if ((rc = check_device())) return rc;
+  if ((rc = use_device(device))) return rc;
   StreamState *st = new StreamState();
   st->cfg = *cfg; st->device = device; st->frames = 0; st->arena = nullptr; st->state = nullptr;
   st->arena_cap = 1 + cfg->beam_size * 256;
@@ -1145,13 +1293,9 @@ static int grow_arenas(void *const *states, int B, const int *clen, cudaStream_t
 struct ChunkBuffers {
   const void *chunk;  // [B, T, V]: probabilities / log-probabilities (kind IN_F32) or logits
   int kind;
-  float *lp;          // the plan's pruned rows and characters (a workspace laid out by the plan, up to off_arena)
-  uint16_t *idx;
+  unsigned char *ws;  // the plan's pruned rows and characters (a workspace laid out by the plan, up to off_arena)
   unsigned char *tab; // stream_tab_layout(B).total bytes
-  int32_t *tokens, *timesteps;  // [B, K, out_T]
-  float *scores;                // [B, K]
-  int32_t *lens;                // [B, K]
-  int32_t *n_results, *flags;   // [B]
+  DecodeOut out;
   int out_T;
 };
 
@@ -1164,13 +1308,14 @@ struct ChunkBuffers {
 static int stream_chunk_step(const ctcdec_config &cfg, Plan &pl, void *const *states, int B, int T,
                              const int32_t *seq_lens, const uint8_t *is_eos, const ChunkBuffers &io, DevCache *c,
                              cudaStream_t s) {
-  const int V = cfg.vocab_size, K = cfg.beam_size;
   int rc = CTCDEC_OK;
   bool any_eos = false;
   std::vector<int> clen(B);
+  std::vector<uint8_t> at_root(B);  // streams that have not seen a frame yet
   for (int b = 0; b < B; ++b) {
     clen[b] = std::max(0, std::min(seq_lens ? seq_lens[b] : T, T));
     any_eos |= is_eos[b] != 0;
+    at_root[b] = static_cast<StreamState *>(states[b])->frames == 0;
   }
   if ((rc = grow_arenas(states, B, clen.data(), s))) return rc;
   HostScorer *const sc = static_cast<StreamState *>(states[0])->sc;
@@ -1189,65 +1334,34 @@ static int stream_chunk_step(const ctcdec_config &cfg, Plan &pl, void *const *st
     CU(cudaGetLastError());
   }
   const int *d_len = seq_lens ? reinterpret_cast<const int *>(io.tab + L.lens) : nullptr;
-  CU(cudaMemsetAsync(io.flags, 0, (size_t)B * 4, s));
-  CU(cudaMemsetAsync(io.n_results, 0, (size_t)B * 4, s));
-  if (T > 0 && (rc = launch_prune(&cfg, pl, PruneInput{io.chunk, io.kind, nullptr, sc != nullptr}, d_len, B, T, io.lp,
-                                  io.idx, io.flags, s)))
+  CU(cudaMemsetAsync(io.out.flags, 0, (size_t)B * 4, s));
+  CU(cudaMemsetAsync(io.out.n_results, 0, (size_t)B * 4, s));
+  if (T > 0 && (rc = launch_prune(&cfg, pl, PruneInput{io.chunk, io.kind, nullptr, sc != nullptr}, d_len, B, T, io.ws,
+                                  io.out.flags, s)))
     return rc;
-  BeamParams bp;
-  memset(&bp, 0, sizeof(bp));
-  bp.lp = io.lp; bp.idx = io.idx; bp.seq_lens = d_len; bp.T = T; bp.V = V; bp.NP = pl.NP; bp.K = K;
-  bp.blank = cfg.blank_id; bp.tile_frames = pl.F;
+  BeamParams bp = beam_params(cfg, pl, io.ws, d_len, T, io.out, io.out_T);
+  bp.tile_frames = pl.F;
   bp.arena_ptrs = (Node *const *)(io.tab + L.arenas); bp.state_ptrs = (int *const *)(io.tab + L.states);
   bp.arena_caps = (const int *)(io.tab + L.caps);
   bp.finalize = io.tab + L.fin;
   bp.fresh = 0;
-  bp.out_tokens = io.tokens; bp.out_timesteps = io.timesteps; bp.out_scores = io.scores; bp.out_lens = io.lens;
-  bp.n_results = io.n_results; bp.out_T = io.out_T; bp.flags = io.flags;
-  if (sc && sc->ngram && T > 0) {
-    // ARPA scorer: the beam kernel computes the LM terms itself, one launch per chunk and no handshake
-    if ((rc = ensure_ngram_on_device(sc, static_cast<StreamState *>(states[0])->device))) return rc;
-    bp.dict_next = sc->d_next; bp.dict_mask = sc->d_mask; bp.dict_wc = sc->dict.wc; bp.dict_start = sc->dict.start;
-    bp.space_id = sc->space_id; bp.beta = sc->beta;
+  if (sc && T > 0) {
+    if (sc->ngram && (rc = ensure_ngram_on_device(sc, static_cast<StreamState *>(states[0])->device))) return rc;
+    attach_scorer(bp, *sc);
     bp.lm_arena_ptrs = (float *const *)(io.tab + L.lmar);
     bp.dstate_ptrs = (int *const *)(io.tab + L.dst);
-    if (sc->is_character_based) { bp.lm_char = 1; bp.lm_row_ptrs = (float *const *)(io.tab + L.rows); }
-    bp.lm_dev = 1; bp.lm_alpha = sc->alpha; bp.ngram = sc->d_view;
-    bp.word_of_state = sc->d_word_of_state; bp.label_word = sc->d_label_word; bp.lm_hist_n = sc->max_order - 1;
-    if ((rc = launch_beam(bp, pl, B, s))) return rc;
-  } else if (sc && T > 0) {
-    // scorer path: one persistent launch per chunk, hand shake after EVERY frame (the frame after the chunk's last
-    // one, in the next call, needs the LM terms of the nodes created now)
-    int nls = 0, ups = 0;
-    exchange_strides(K, exchange_row_len(*sc), &nls, &ups);
-    if ((rc = ensure_pinned(*c, 0, (size_t)B * nls * 4))) return rc;
-    if ((rc = ensure_pinned(*c, 1, (size_t)B * ups * 4))) return rc;
-    if ((rc = ensure_pinned(*c, 2, 256))) return rc;
-    int *h_newlist = (int *)c->pin[0], *h_upd = (int *)c->pin[1], *hs_abort = (int *)c->pin[2];
-    for (int b = 0; b < B; ++b) { memset(h_newlist + (size_t)b * nls, 0, 16); memset(h_upd + (size_t)b * ups, 0, 8); }
-    if (sc->is_character_based) {  // streams that have not seen a frame yet: the root's row of LM terms first
-      std::vector<int> scratch;
-      for (int b = 0; b < B; ++b)
-        if (static_cast<StreamState *>(states[b])->frames == 0)
-          lm_char_root_entry(*sc, sc->cond_caches[0], h_upd + (size_t)b * ups, scratch);
-      bp.lm_char = 1;
-      bp.lm_row_ptrs = (float *const *)(io.tab + L.rows);
-    }
-    *hs_abort = 0;
-    bp.dict_next = sc->d_next; bp.dict_mask = sc->d_mask; bp.dict_wc = sc->dict.wc; bp.dict_start = sc->dict.start;
-    bp.space_id = sc->space_id; bp.beta = sc->beta;
-    bp.lm_arena_ptrs = (float *const *)(io.tab + L.lmar);
-    bp.dstate_ptrs = (int *const *)(io.tab + L.dst);
-    bp.newlist = h_newlist; bp.lm_upd = h_upd; bp.lm_nl_stride = nls; bp.lm_up_stride = ups;
-    bp.lm_persistent = 1; bp.lm_hs_last = 1; bp.hs_abort = hs_abort;
-    if ((rc = launch_beam(bp, pl, B, s))) return rc;
+    if (sc->is_character_based) bp.lm_row_ptrs = (float *const *)(io.tab + L.rows);
+  }
+  if (sc && !sc->ngram && T > 0) {
+    // hook scorer: one persistent launch per chunk, hand shake after EVERY frame (the frame after the chunk's last
+    // one, in the next call, needs the LM terms of the nodes created now).  An n-gram scorer needs none: the beam
+    // kernel computes the LM terms itself.
+    if ((rc = prepare_exchange(*c, *sc, B, at_root.data(), bp))) return rc;
+    bp.lm_hs_last = 1;
     std::vector<TrieMirror *> mirrors(B);
     for (int b = 0; b < B; ++b) mirrors[b] = &static_cast<StreamState *>(states[b])->mirror;
-    const int failed = serve_handshakes(sc, B, K, clen.data(), mirrors.data(), h_newlist, h_upd, nullptr);
-    if (failed) reinterpret_cast<std::atomic<int> *>(hs_abort)->store(1, std::memory_order_release);
-    const cudaError_t e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) return fail(CTCDEC_E_CUDA, "beam kernel (scorer path, streaming): %s", cudaGetErrorString(e));
-    if (failed) return fail(CTCDEC_E_CUDA, "beam kernel (scorer path, streaming) stopped answering the per-frame handshake");
+    if ((rc = run_handshake(bp, pl, B, sc, *c, clen.data(), mirrors.data(), nullptr, "scorer path, streaming", s)))
+      return rc;
   } else if (T > 0 && (rc = launch_beam(bp, pl, B, s))) {
     return rc;
   }
@@ -1268,8 +1382,7 @@ int ctcdec_decode_stream_host(const float *probs, const int32_t *seq_lens, int B
   Plan pl;
   if ((rc = make_plan(&cfg, B, T, &pl, s0->sc != nullptr))) return rc;
   const int device = s0->device;
-  if (cudaSetDevice(device) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "cudaSetDevice(%d) failed", device);
-  if ((rc = check_device())) return rc;
+  if ((rc = use_device(device))) return rc;
   std::lock_guard<std::mutex> lock(g_mu[device]);
   DevCache &c = g_cache[device];
   if (!c.stream) CU(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
@@ -1280,69 +1393,52 @@ int ctcdec_decode_stream_host(const float *probs, const int32_t *seq_lens, int B
   for (int b = 0; b < B; ++b) any_eos |= is_eos[b] != 0;
   if (any_eos && (!tokens || !timesteps || !scores || !lens)) return fail(CTCDEC_E_INVALID, "an output pointer is NULL");
   if (any_eos && out_T < 0) return fail(CTCDEC_E_INVALID, "out_T < 0");
-  const size_t n_probs = (size_t)B * T * V, n_bk = (size_t)B * K, n_out = any_eos ? n_bk * (size_t)out_T : 0;
+  const size_t n_probs = (size_t)B * T * V, n_out = any_eos ? (size_t)B * K * (size_t)out_T : 0;
   HostScorer *const sc = s0->sc;
-  if ((rc = ensure(c, 0, n_probs * 4 + 256))) return rc;
-  if ((rc = ensure(c, 2, n_out * 4 + 256))) return rc;
-  if ((rc = ensure(c, 3, n_out * 4 + 256))) return rc;
-  if ((rc = ensure(c, 4, n_bk * 4 * 2 + (size_t)B * 8 + 1024))) return rc;
-  if ((rc = ensure(c, 5, pl.off_arena + 512))) return rc;  // only the lp / idx part of the plan is used
-  if ((rc = ensure(c, 6, stream_tab_layout(B).total + 256))) return rc;
-  float *d_probs = (float *)c.buf[0];
-  int *d_tok = (int *)c.buf[2], *d_ts = (int *)c.buf[3];
-  float *d_scores = (float *)c.buf[4];
-  int *d_lens = (int *)((char *)c.buf[4] + al256(n_bk * 4));
-  int *d_nres = (int *)((char *)d_lens + al256(n_bk * 4));
-  int *d_flags = d_nres + B;
+  if ((rc = ensure(c, kBufInput, n_probs * 4 + 256))) return rc;
+  if ((rc = ensure(c, kBufTokens, n_out * 4 + 256))) return rc;
+  if ((rc = ensure(c, kBufTimesteps, n_out * 4 + 256))) return rc;
+  if ((rc = ensure(c, kBufSmall, small_bytes(B, K)))) return rc;
+  if ((rc = ensure(c, kBufWork, pl.off_arena + 512))) return rc;  // only the lp / idx part of the plan is used
+  if ((rc = ensure(c, kBufStreamTab, stream_tab_layout(B).total + 256))) return rc;
+  float *d_probs = (float *)c.buf[kBufInput];
+  int *d_tok = (int *)c.buf[kBufTokens], *d_ts = (int *)c.buf[kBufTimesteps];
+  const SmallOut d = small_out(c.buf[kBufSmall], B, K);
   if (n_probs) CU(cudaMemcpyAsync(d_probs, probs, n_probs * 4, cudaMemcpyHostToDevice, s));
-  unsigned char *ws = (unsigned char *)c.buf[5];
-  ws = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(ws) + 255) / 256 * 256);
   ChunkBuffers io;
   io.chunk = d_probs; io.kind = IN_F32;
-  io.lp = reinterpret_cast<float *>(ws + pl.off_lp);
-  io.idx = pl.sorted ? reinterpret_cast<uint16_t *>(ws + pl.off_idx) : nullptr;
-  io.tab = (unsigned char *)c.buf[6];
-  io.tokens = d_tok; io.timesteps = d_ts; io.scores = d_scores; io.lens = d_lens; io.n_results = d_nres;
-  io.flags = d_flags; io.out_T = out_T;
+  io.ws = align256(c.buf[kBufWork]);
+  io.tab = (unsigned char *)c.buf[kBufStreamTab];
+  io.out = DecodeOut{d_tok, d_ts, d.scores, d.lens, d.n_results, d.flags};
+  io.out_T = out_T;
   if ((rc = stream_chunk_step(cfg, pl, states, B, T, seq_lens, is_eos, io, &c, s))) return rc;
   if (any_eos) {
-    std::unique_ptr<int[]> h_nres(new int[(size_t)B * 2]);
-    std::unique_ptr<float[]> h_scores(new float[n_bk]);
-    std::unique_ptr<int[]> h_lens(new int[n_bk]);
-    CU(cudaMemcpyAsync(h_scores.get(), d_scores, n_bk * 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(h_lens.get(), d_lens, n_bk * 4, cudaMemcpyDeviceToHost, s));
-    CU(cudaMemcpyAsync(h_nres.get(), d_nres, (size_t)B * 8, cudaMemcpyDeviceToHost, s));
+    if ((rc = ensure_pinned(c, kPinSmall, small_bytes(B, K)))) return rc;
+    const SmallOut h = small_out(c.pin[kPinSmall], B, K);
+    if ((rc = read_small(h, d, K, 0, B, s))) return rc;
     CU(cudaStreamSynchronize(s));
-    int max_len = 0;
-    for (int b = 0; b < B; ++b) {
-      if (!is_eos[b]) continue;
-      for (int p = 0; p < h_nres[b] && p < K; ++p) {
-        scores[(size_t)b * K + p] = h_scores[(size_t)b * K + p];
-        lens[(size_t)b * K + p] = h_lens[(size_t)b * K + p];
-        max_len = std::max(max_len, h_lens[(size_t)b * K + p]);
-      }
-    }
+    copy_result_rows(h, B, K, is_eos, scores, lens);
+    const int max_len = max_result_len(h, K, 0, B, is_eos);
     if (max_len > out_T) return fail(CTCDEC_E_INVALID, "out_T (%d) smaller than the longest prefix (%d)", out_T, max_len);
     if (max_len > 0) {
       // copy per finalized stream so rows of non-eos streams stay untouched
       for (int b = 0; b < B; ++b) {
-        if (!is_eos[b] || h_nres[b] == 0) continue;
+        if (!is_eos[b] || h.n_results[b] == 0) continue;
         const size_t off = (size_t)b * K * out_T;
-        CU(cudaMemcpy2DAsync(tokens + off, (size_t)out_T * 4, d_tok + off, (size_t)out_T * 4, (size_t)max_len * 4,
-                             (size_t)h_nres[b], cudaMemcpyDeviceToHost, s));
-        CU(cudaMemcpy2DAsync(timesteps + off, (size_t)out_T * 4, d_ts + off, (size_t)out_T * 4, (size_t)max_len * 4,
-                             (size_t)h_nres[b], cudaMemcpyDeviceToHost, s));
+        if ((rc = enqueue_rows(d_tok + off, d_ts + off, tokens + off, timesteps + off, nullptr, nullptr,
+                               (size_t)h.n_results[b], max_len, out_T, s)))
+          return rc;
       }
     }
     CU(cudaStreamSynchronize(s));
     if (sc) {  // reported scores of the finished streams: approx_ctc (reference ctc_beam_search_decoder.cpp:173-208)
       std::vector<int> nres_eos(B);
-      for (int b = 0; b < B; ++b) nres_eos[b] = is_eos[b] ? h_nres[b] : 0;
+      for (int b = 0; b < B; ++b) nres_eos[b] = is_eos[b] ? h.n_results[b] : 0;
       lm_rescore_batch(*sc, B, K, out_T, nres_eos.data(), tokens, lens, scores);
     }
-    if (n_results) memcpy(n_results, h_nres.get(), (size_t)B * 4);
-    if (flags) memcpy(flags, h_nres.get() + B, (size_t)B * 4);
-    if ((rc = check_error_flags(h_nres.get() + B, B))) return rc;
+    if (n_results) memcpy(n_results, h.n_results, (size_t)B * 4);
+    if (flags) memcpy(flags, h.flags, (size_t)B * 4);
+    if ((rc = check_error_flags(h.flags, B))) return rc;
   } else {
     CU(cudaStreamSynchronize(s));
     if (n_results) memset(n_results, 0, (size_t)B * 4);
@@ -1365,9 +1461,10 @@ int ctcdec_stream_workspace_bytes(const ctcdec_config *cfg, int B, int T, size_t
 // the states' device must be the current one: the caller's stream and buffers belong to it
 static int check_current_device(const StreamState *s0) {
   int dev = -1;
-  if (cudaGetDevice(&dev) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "no CUDA device (this library has no CPU fallback)");
+  const int rc = current_device(&dev);
+  if (rc) return rc;
   if (dev != s0->device) return fail(CTCDEC_E_INVALID, "the states live on device %d, the current device is %d", s0->device, dev);
-  return check_device();
+  return CTCDEC_OK;
 }
 
 int ctcdec_decode_stream_device(const void *probs, int dtype, const int32_t *seq_lens, int B, int T,
@@ -1375,13 +1472,11 @@ int ctcdec_decode_stream_device(const void *probs, int dtype, const int32_t *seq
                                 int out_T, float *scores, int32_t *lens, int32_t *n_results, int32_t *flags,
                                 void *workspace, size_t workspace_bytes, void *stream) {
   if (B <= 0) return B == 0 ? CTCDEC_OK : fail(CTCDEC_E_INVALID, "negative batch");
-  if (dtype != -1 && dtype != CTCDEC_DTYPE_F32 && dtype != CTCDEC_DTYPE_F16 && dtype != CTCDEC_DTYPE_BF16)
-    return fail(CTCDEC_E_INVALID, "dtype %d is not -1 (probabilities) or one of CTCDEC_DTYPE_F32 / F16 / BF16", dtype);
-  const int kind = dtype == -1 ? IN_F32 : dtype == CTCDEC_DTYPE_F32 ? IN_LOGITS_F32
-                 : dtype == CTCDEC_DTYPE_F16 ? IN_LOGITS_F16 : IN_LOGITS_BF16;
-  if (!states || !is_eos) return fail(CTCDEC_E_INVALID, "states / is_eos is NULL");
-  int rc = check_states(states, B);
+  int kind = 0;
+  int rc = input_kind(dtype, true, &kind);
   if (rc) return rc;
+  if (!states || !is_eos) return fail(CTCDEC_E_INVALID, "states / is_eos is NULL");
+  if ((rc = check_states(states, B))) return rc;
   StreamState *s0 = static_cast<StreamState *>(states[0]);
   HostScorer *const sc = s0->sc;
   if (sc && !sc->ngram)
@@ -1401,20 +1496,17 @@ int ctcdec_decode_stream_device(const void *probs, int dtype, const int32_t *seq
   }
   if (any_eos && (!tokens || !timesteps || !scores || !lens)) return fail(CTCDEC_E_INVALID, "an output pointer is NULL");
   if ((rc = check_current_device(s0))) return rc;
-  unsigned char *ws = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(workspace) + 255) / 256 * 256);
-  const size_t need = stream_workspace_bytes(pl, B);
-  if (!workspace || workspace_bytes < need)
-    return fail(CTCDEC_E_WORKSPACE, "workspace of %zu bytes given, %zu needed", workspace_bytes, need);
+  unsigned char *ws = nullptr;
+  if ((rc = workspace_start(workspace, workspace_bytes, stream_workspace_bytes(pl, B), &ws))) return rc;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   std::lock_guard<std::mutex> lock(g_mu[s0->device]);
   if ((rc = wait_device_work(states, B, s))) return rc;
   ChunkBuffers io;
   io.chunk = probs; io.kind = kind;
-  io.lp = reinterpret_cast<float *>(ws + pl.off_lp);
-  io.idx = pl.sorted ? reinterpret_cast<uint16_t *>(ws + pl.off_idx) : nullptr;
+  io.ws = ws;
   io.tab = ws + al256(pl.off_arena);
-  io.tokens = tokens; io.timesteps = timesteps; io.scores = scores; io.lens = lens; io.n_results = n_results;
-  io.flags = flags; io.out_T = out_T;
+  io.out = DecodeOut{tokens, timesteps, scores, lens, n_results, flags};
+  io.out_T = out_T;
   if ((rc = stream_chunk_step(cfg, pl, states, B, T, seq_lens, is_eos, io, nullptr, s))) return rc;
   if (sc && any_eos) {  // the eos streams' reported scores (the other streams' n_results are 0: their rows are skipped)
     if ((rc = ensure_ngram_on_device(sc, s0->device))) return rc;
@@ -1438,7 +1530,7 @@ int ctcdec_stream_committed_device(void *const *states, int B, const int32_t *si
   std::lock_guard<std::mutex> lock(g_mu[s0->device]);
   if ((rc = wait_device_work(states, B, s))) return rc;
   const size_t smem = committed_smem_bytes(K);
-  if (smem > 48 * 1024) CU(cudaFuncSetAttribute(committed_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if ((rc = raise_smem_limit<committed_kernel<128>>(smem, "committed-prefix"))) return rc;
   for (int b0 = 0; b0 < B; b0 += kCommitPerLaunch) {
     CommitArgs a;
     memset(&a, 0, sizeof(a));
@@ -1585,9 +1677,7 @@ struct LmBuffers {
   int *dstate;                   // [B][arena_stride] dictionary state of each trie node
   float *lm_row;                 // character-based model: [B][arena_stride][V] rows of LM terms, else NULL
   int *lm_hist;                  // ARPA scorer: [B][arena_stride][order - 1] LM word ids of each trie node, else NULL
-  int32_t *tokens, *timesteps;   // [B, K, T]
-  float *scores;                 // [B, K] (the raw prefix scores: the caller rescores them with lm_rescore_batch)
-  int32_t *lens, *n_results, *flags;
+  DecodeOut out;                 // (scores: the raw prefix scores, which the caller rescores)
   // sweep of the LM weights (ARPA scorer): P pairs (alpha, beta) in the device table lm_ab [P][2]; the per-node arrays
   // and the outputs above then hold P x B utterances (pair-major), the input rows B
   int P = 1;
@@ -1603,63 +1693,33 @@ struct LmBuffers {
 // caller holds g_mu[device].
 static int lm_batch_step(const ctcdec_config *cfg, const Plan &pl, HostScorer *sc, DevCache &c, int device,
                          const int32_t *seq_lens, int B, int T, const LmBuffers &io, cudaStream_t s) {
-  const int V = cfg->vocab_size, K = cfg->beam_size;
+  const int K = cfg->beam_size;
   int rc = ensure_dict_on_device(sc, device);
   if (rc || (sc->ngram && (rc = ensure_ngram_on_device(sc, device)))) return rc;
-  const bool lm_char = sc->is_character_based != 0;
   const int G = io.P * B;  // beam CTAs
-  CU(cudaMemsetAsync(io.flags, 0, (size_t)G * 4, s));
-  float *lp = reinterpret_cast<float *>(io.ws + pl.off_lp);
-  uint16_t *idx = pl.sorted ? reinterpret_cast<uint16_t *>(io.ws + pl.off_idx) : nullptr;
-  if ((rc = launch_prune(cfg, pl, io.in, io.seq_lens, B, T, lp, idx, io.flags, s))) return rc;
+  CU(cudaMemsetAsync(io.out.flags, 0, (size_t)G * 4, s));
+  if ((rc = launch_prune(cfg, pl, io.in, io.seq_lens, B, T, io.ws, io.out.flags, s))) return rc;
   if (io.P > 1) {
     const long long n = (long long)(io.P - 1) * B;
-    sweep_flags_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(io.flags, B, n);
+    sweep_flags_kernel<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(io.out.flags, B, n);
     CU(cudaGetLastError());
   }
 
-  BeamParams bp;
-  memset(&bp, 0, sizeof(bp));
-  bp.lp = lp; bp.idx = idx; bp.seq_lens = io.seq_lens; bp.T = T; bp.V = V; bp.NP = pl.NP; bp.K = K;
-  bp.blank = cfg->blank_id; bp.tile_frames = 1;
-  bp.arena = reinterpret_cast<Node *>(io.ws + pl.off_arena); bp.arena_stride = pl.arena_stride;
-  bp.state = reinterpret_cast<int *>(io.ws + pl.off_state); bp.state_stride = pl.state_stride;
-  bp.arena_cap = (int)pl.arena_stride;
-  bp.out_tokens = io.tokens; bp.out_timesteps = io.timesteps; bp.out_scores = io.scores; bp.out_lens = io.lens;
-  bp.n_results = io.n_results; bp.out_T = T; bp.flags = io.flags;
-  bp.force_fallback = getenv("CTCDEC_FORCE_FALLBACK") ? 1 : 0;
-  bp.dict_next = sc->d_next; bp.dict_mask = sc->d_mask; bp.dict_wc = sc->dict.wc; bp.dict_start = sc->dict.start;
-  bp.space_id = sc->space_id; bp.beta = sc->beta; bp.lm_arena = io.lm_arena; bp.dstate_arena = io.dstate;
-  bp.lm_char = lm_char ? 1 : 0; bp.lm_row = lm_char ? io.lm_row : nullptr;
-  bp.timing = g_prof.timing;
+  BeamParams bp = beam_params(*cfg, pl, io.ws, io.seq_lens, T, io.out, T);
+  flat_arenas(bp, pl, io.ws);
+  bp.tile_frames = 1; bp.fresh = 1;
+  attach_scorer(bp, *sc);
+  bp.lm_arena = io.lm_arena; bp.dstate_arena = io.dstate; bp.lm_row = io.lm_row;
   if (sc->ngram) {
     // ARPA scorer: the beam kernel computes the LM terms itself, so ONE launch decodes the batch, with no exchange
     // blocks, host workers or handshake
-    bp.lm_dev = 1; bp.lm_alpha = sc->alpha; bp.ngram = sc->d_view;
-    bp.word_of_state = sc->d_word_of_state; bp.label_word = sc->d_label_word;
-    bp.lm_hist_n = sc->max_order - 1; bp.lm_hist = io.lm_hist;
+    bp.lm_hist = io.lm_hist;
     bp.sweep_B = io.lm_ab ? B : 0; bp.lm_ab = io.lm_ab;
-    bp.t0 = 0; bp.nframes = 0; bp.fresh = 1;
     if ((rc = launch_beam(bp, pl, G, s))) return rc;
     return launch_finalize(bp, G, s);
   }
-  int nls = 0, ups = 0;
-  exchange_strides(K, exchange_row_len(*sc), &nls, &ups);
-  if ((rc = ensure_pinned(c, 0, (size_t)B * nls * 4))) return rc;
-  if ((rc = ensure_pinned(c, 1, (size_t)B * ups * 4))) return rc;
-  if ((rc = ensure_pinned(c, 2, 256))) return rc;
-  int *h_newlist = (int *)c.pin[0], *h_upd = (int *)c.pin[1], *hs_abort = (int *)c.pin[2];
-  for (int b = 0; b < B; ++b) { memset(h_newlist + (size_t)b * nls, 0, 16); memset(h_upd + (size_t)b * ups, 0, 8); }
-  if (lm_char) {  // the root's row of LM terms: the first entry every CTA picks up before frame 0
-    std::vector<int> scratch;
-    lm_char_root_entry(*sc, sc->cond_caches[0], h_upd, scratch);
-    for (int b = 1; b < B; ++b) memcpy(h_upd + (size_t)b * ups, h_upd, (size_t)(3 + V) * 4);
-  }
-  *hs_abort = 0;
-  // The per-frame exchange with the host goes through pinned, device-mapped host memory (unified addressing):
-  // the kernel reads the few LM updates and writes the new-node list straight over PCIe, so a frame costs one
-  // launch and one stream synchronisation, no memcpy calls.
-  bp.newlist = h_newlist; bp.lm_upd = h_upd; bp.lm_nl_stride = nls; bp.lm_up_stride = ups;
+  if ((rc = prepare_exchange(c, *sc, B, nullptr, bp))) return rc;
+  int *const h_newlist = (int *)c.pin[kPinNewList], *const h_upd = (int *)c.pin[kPinUpdates];
   std::vector<int> need(B);
   int tmax = 0;
   for (int b = 0; b < B; ++b) {
@@ -1670,32 +1730,14 @@ static int lm_batch_step(const ctcdec_config *cfg, const Plan &pl, HostScorer *s
   for (int b = 0; b < B; ++b) mirror[b].reserve((size_t)1 + (size_t)K * need[b]);
   const bool lm_timing = getenv("CTCDEC_LM_TIMING") != nullptr;
   if (getenv("CTCDEC_LM_PER_FRAME") == nullptr) {
-    // ---- persistent mode (default): ONE launch decodes every utterance start to end.  After each frame a CTA
-    // publishes its new nodes in mapped host memory, raises its done flag and polls its go flag; host workers (each
-    // owning every nt-th utterance, with its own hook cache) answer with the LM terms.  CTAs never wait on each
-    // other, so the scheme needs no co-residency; a kernel-side deadline and the abort flag bound every wait.
-    bp.lm_persistent = 1; bp.hs_abort = hs_abort;
-    bp.t0 = 0; bp.nframes = 0; bp.fresh = 1;
+    // ---- persistent mode (default): ONE launch decodes every utterance start to end; host workers (each owning
+    // every nt-th utterance, with its own hook cache) answer each frame with the LM terms.
     const auto c0 = std::chrono::steady_clock::now();
-    if (!c.beam_ev) CU(cudaEventCreateWithFlags(&c.beam_ev, cudaEventDisableTiming));
-    CU(cudaEventRecord(c.beam_ev, s));
-    if ((rc = launch_beam(bp, pl, B, s))) return rc;
-    // the handshake gives up after 8 s without progress: start its clock once the work queued on s before the beam
-    // kernel (the caller's, on a stream of the caller's) has finished
-    const cudaError_t ew = cudaEventSynchronize(c.beam_ev);
-    if (ew != cudaSuccess) {
-      reinterpret_cast<std::atomic<int> *>(hs_abort)->store(1, std::memory_order_release);
-      return fail(CTCDEC_E_CUDA, "work queued before the beam kernel (scorer path): %s", cudaGetErrorString(ew));
-    }
     std::vector<TrieMirror *> mirrors(B);
     std::vector<int> answers(B);
     for (int b = 0; b < B; ++b) { mirrors[b] = &mirror[b]; answers[b] = std::max(0, need[b] - 1); }
     HandshakeStats hst;
-    const int failed = serve_handshakes(sc, B, K, answers.data(), mirrors.data(), h_newlist, h_upd, &hst);
-    if (failed) reinterpret_cast<std::atomic<int> *>(hs_abort)->store(1, std::memory_order_release);
-    const cudaError_t e = cudaStreamSynchronize(s);
-    if (e != cudaSuccess) return fail(CTCDEC_E_CUDA, "beam kernel (scorer path): %s", cudaGetErrorString(e));
-    if (failed) return fail(CTCDEC_E_CUDA, "beam kernel (scorer path) stopped answering the per-frame handshake");
+    if ((rc = run_handshake(bp, pl, B, sc, c, answers.data(), mirrors.data(), &hst, "scorer path", s))) return rc;
     if (lm_timing)
       fprintf(stderr, "[ctcdec lm] persistent: frames %d, %u host workers, kernel+handshakes %.1f ms (%lld hook calls, %lld new nodes)\n",
               tmax, hst.workers, std::chrono::duration<double>(std::chrono::steady_clock::now() - c0).count() * 1e3,
@@ -1712,9 +1754,9 @@ static int lm_batch_step(const ctcdec_config *cfg, const Plan &pl, HostScorer *s
       CU(cudaStreamSynchronize(s));
       const auto c1 = std::chrono::steady_clock::now();
       for (int b = 0; b < B; ++b) {
-        n_hook += lm_after_frame(*sc, sc->cond_caches[0], mirror[b], h_newlist + (size_t)b * nls,
-                                 h_upd + (size_t)b * ups, scratch);
-        n_new += h_newlist[(size_t)b * nls];
+        int *const nl = h_newlist + (size_t)b * bp.lm_nl_stride;
+        n_hook += lm_after_frame(*sc, sc->cond_caches[0], mirror[b], nl, h_upd + (size_t)b * bp.lm_up_stride, scratch);
+        n_new += nl[0];
       }
       const auto c2 = std::chrono::steady_clock::now();
       t_gpu += std::chrono::duration<double>(c1 - c0).count();
@@ -1727,110 +1769,9 @@ static int lm_batch_step(const ctcdec_config *cfg, const Plan &pl, HostScorer *s
   return launch_finalize(bp, B, s);
 }
 
-int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const float *probs, const int32_t *seq_lens,
-                                int B, int T, int32_t *tokens, int32_t *timesteps, float *scores, int32_t *lens,
-                                int32_t *n_results, int32_t *flags, int device) {
-  if (!scorer) return fail(CTCDEC_E_INVALID, "scorer is NULL");
-  const auto t_call0 = std::chrono::steady_clock::now();
-  HostScorer *sc = static_cast<HostScorer *>(scorer);
-  Plan pl;
-  int rc = make_plan(cfg, B, T, &pl, true);
-  if (rc) return rc;
-  if ((int)sc->labels.size() != cfg->vocab_size) return fail(CTCDEC_E_INVALID, "scorer was built for %zu labels, decoder has %d", sc->labels.size(), cfg->vocab_size);
-  if (device < 0 || device >= 64) return fail(CTCDEC_E_INVALID, "device %d out of range", device);
-  if (cudaSetDevice(device) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "cudaSetDevice(%d) failed (this library has no CPU fallback)", device);
-  if ((rc = check_device())) return rc;
-  if (B == 0) return CTCDEC_OK;
-  std::lock_guard<std::mutex> lock(g_mu[device]);
-  DevCache &c = g_cache[device];
-  if (!c.stream) CU(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
-  cudaStream_t s = c.stream;
-  const int V = cfg->vocab_size, K = cfg->beam_size;
-  const size_t n_probs = (size_t)B * T * V, n_out = (size_t)B * K * T, n_bk = (size_t)B * K;
-  const size_t lm_bytes = al256((size_t)B * pl.arena_stride * 4) * 2;
-  size_t row_bytes = 0;
-  if ((rc = lm_row_bytes(sc, pl, B, &row_bytes))) return rc;
-  size_t hist_bytes = 0;
-  if ((rc = lm_hist_bytes(sc, pl, B, &hist_bytes))) return rc;
-  if ((rc = ensure(c, 0, n_probs * 4 + 256))) return rc;
-  if ((rc = ensure(c, 1, (size_t)B * 4 + 256))) return rc;
-  if ((rc = ensure(c, 2, n_out * 4 + 256))) return rc;
-  if ((rc = ensure(c, 3, n_out * 4 + 256))) return rc;
-  if ((rc = ensure(c, 4, n_bk * 4 * 2 + (size_t)B * 8 + 1024))) return rc;
-  if ((rc = ensure(c, 5, pl.total + 512))) return rc;
-  if ((rc = ensure(c, 7, lm_bytes + 512))) return rc;
-  if (row_bytes && (rc = ensure(c, 8, row_bytes + 256))) return rc;
-  if (hist_bytes && (rc = ensure(c, 9, hist_bytes + 256))) return rc;
-  float *d_probs = (float *)c.buf[0];
-  int *d_lens_in = seq_lens ? (int *)c.buf[1] : nullptr;
-  int *d_tok = (int *)c.buf[2], *d_ts = (int *)c.buf[3];
-  float *d_scores = (float *)c.buf[4];
-  int *d_lens = (int *)((char *)c.buf[4] + al256(n_bk * 4));
-  int *d_nres = (int *)((char *)d_lens + al256(n_bk * 4));
-  int *d_flags = d_nres + B;
-  unsigned char *lmb = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(c.buf[7]) + 255) / 256 * 256);
-  if (n_probs) CU(cudaMemcpyAsync(d_probs, probs, n_probs * 4, cudaMemcpyHostToDevice, s));
-  if (seq_lens) CU(cudaMemcpyAsync(d_lens_in, seq_lens, (size_t)B * 4, cudaMemcpyHostToDevice, s));
-  LmBuffers io;
-  io.in = PruneInput{d_probs, IN_F32, nullptr, true};
-  io.seq_lens = d_lens_in;
-  io.ws = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(c.buf[5]) + 255) / 256 * 256);
-  io.lm_arena = (float *)lmb;
-  io.dstate = (int *)(lmb + al256((size_t)B * pl.arena_stride * 4));
-  io.lm_row = row_bytes ? (float *)c.buf[8] : nullptr;
-  io.lm_hist = hist_bytes ? (int *)c.buf[9] : nullptr;
-  io.tokens = d_tok; io.timesteps = d_ts; io.scores = d_scores; io.lens = d_lens; io.n_results = d_nres;
-  io.flags = d_flags;
-  if ((rc = lm_batch_step(cfg, pl, sc, c, device, seq_lens, B, T, io, s))) return rc;
-  const bool lm_timing = getenv("CTCDEC_LM_TIMING") != nullptr;
-  const auto t_fin0 = std::chrono::steady_clock::now();
-  std::unique_ptr<int[]> h_nres(new int[(size_t)B * 2]);
-  std::unique_ptr<float[]> h_scores(new float[n_bk]);
-  std::unique_ptr<int[]> h_lens(new int[n_bk]);
-  CU(cudaMemcpyAsync(h_scores.get(), d_scores, n_bk * 4, cudaMemcpyDeviceToHost, s));
-  CU(cudaMemcpyAsync(h_lens.get(), d_lens, n_bk * 4, cudaMemcpyDeviceToHost, s));
-  CU(cudaMemcpyAsync(h_nres.get(), d_nres, (size_t)B * 8, cudaMemcpyDeviceToHost, s));
-  CU(cudaStreamSynchronize(s));
-  int max_len = 0;
-  for (int b = 0; b < B; ++b) {  // rows p >= n_results[b] stay as the caller left them
-    const size_t nr = (size_t)std::max(0, std::min(h_nres[b], K));
-    memcpy(scores + (size_t)b * K, h_scores.get() + (size_t)b * K, nr * 4);
-    memcpy(lens + (size_t)b * K, h_lens.get() + (size_t)b * K, nr * 4);
-  }
-  for (int b = 0; b < B; ++b)
-    for (int p = 0; p < h_nres[b] && p < K; ++p) max_len = std::max(max_len, lens[(size_t)b * K + p]);
-  if (max_len > T) max_len = T;
-  if (max_len > 0) {
-    const size_t st_bytes = n_bk * (size_t)max_len * 8;
-    const bool staged = st_bytes <= kMaxRowStaging && !(host_ptr_is_pinned(tokens) && host_ptr_is_pinned(timesteps));
-    if (staged) {
-      if ((rc = ensure_pinned(c, 5, st_bytes))) return rc;
-      int *const stage_tok = static_cast<int *>(c.pin[5]), *const stage_ts = stage_tok + n_bk * (size_t)max_len;
-      CU(cudaMemcpy2DAsync(stage_tok, (size_t)max_len * 4, d_tok, (size_t)T * 4, (size_t)max_len * 4, n_bk, cudaMemcpyDeviceToHost, s));
-      CU(cudaMemcpy2DAsync(stage_ts, (size_t)max_len * 4, d_ts, (size_t)T * 4, (size_t)max_len * 4, n_bk, cudaMemcpyDeviceToHost, s));
-      CU(cudaStreamSynchronize(s));
-      spread_rows(stage_tok, stage_ts, tokens, timesteps, n_bk, max_len, T);
-    } else {
-      CU(cudaMemcpy2DAsync(tokens, (size_t)T * 4, d_tok, (size_t)T * 4, (size_t)max_len * 4, n_bk, cudaMemcpyDeviceToHost, s));
-      CU(cudaMemcpy2DAsync(timesteps, (size_t)T * 4, d_ts, (size_t)T * 4, (size_t)max_len * 4, n_bk, cudaMemcpyDeviceToHost, s));
-    }
-  }
-  CU(cudaStreamSynchronize(s));
-  const auto t_fin1 = std::chrono::steady_clock::now();
-  lm_rescore_batch(*sc, B, K, T, h_nres.get(), tokens, lens, scores);  // reported scores: approx_ctc (reference :194-208)
-  if (lm_timing)
-    fprintf(stderr, "[ctcdec lm] finalize + copies back %.1f ms, read-out rescoring (sentence hook) %.1f ms, whole call %.1f ms\n",
-            std::chrono::duration<double>(t_fin1 - t_fin0).count() * 1e3,
-            std::chrono::duration<double>(std::chrono::steady_clock::now() - t_fin1).count() * 1e3,
-            std::chrono::duration<double>(std::chrono::steady_clock::now() - t_call0).count() * 1e3);
-  if (n_results) memcpy(n_results, h_nres.get(), (size_t)B * 4);
-  if (flags) memcpy(flags, h_nres.get() + B, (size_t)B * 4);
-  return check_error_flags(h_nres.get() + B, B);
-}
-
-// Device scratch of ctcdec_decode_batch_lm_device: the plan's regions, then the per-node LM terms and dictionary
-// states, for a character-based model the per-node rows of LM terms, for an ARPA scorer the per-node LM histories, and
-// the device copy of seq_lens.
+// Device scratch of a scorer decode (the caller's workspace, or the per-device cache's for ctcdec_decode_batch_lm_host):
+// the plan's regions, then the per-node LM terms and dictionary states, for a character-based model the per-node rows
+// of LM terms, for an ARPA scorer the per-node LM histories, and the device copy of seq_lens.
 struct LmWorkspace { size_t lm_arena, dstate, rows, hist, lens, total; };
 static int lm_workspace(const HostScorer *sc, const Plan &pl, int B, LmWorkspace *w) {
   size_t row_bytes = 0, hist_bytes = 0;
@@ -1844,6 +1785,87 @@ static int lm_workspace(const HostScorer *sc, const Plan &pl, int B, LmWorkspace
   w->lens = w->hist + al256(hist_bytes);
   w->total = w->lens + al256((size_t)B * 4);
   return CTCDEC_OK;
+}
+
+// the buffers of a scorer decode in a workspace laid out by lm_workspace (ws: its aligned start); the caller sets seq_lens
+static LmBuffers lm_buffers(const HostScorer &sc, const LmWorkspace &w, unsigned char *ws, const PruneInput &in,
+                            const DecodeOut &out) {
+  LmBuffers io;
+  io.in = in;
+  io.seq_lens = nullptr;
+  io.ws = ws;
+  io.lm_arena = reinterpret_cast<float *>(ws + w.lm_arena);
+  io.dstate = reinterpret_cast<int *>(ws + w.dstate);
+  io.lm_row = sc.is_character_based ? reinterpret_cast<float *>(ws + w.rows) : nullptr;
+  io.lm_hist = sc.ngram ? reinterpret_cast<int *>(ws + w.hist) : nullptr;
+  io.out = out;
+  return io;
+}
+
+int ctcdec_decode_batch_lm_host(const ctcdec_config *cfg, void *scorer, const float *probs, const int32_t *seq_lens,
+                                int B, int T, int32_t *tokens, int32_t *timesteps, float *scores, int32_t *lens,
+                                int32_t *n_results, int32_t *flags, int device) {
+  if (!scorer) return fail(CTCDEC_E_INVALID, "scorer is NULL");
+  const auto t_call0 = std::chrono::steady_clock::now();
+  HostScorer *sc = static_cast<HostScorer *>(scorer);
+  Plan pl;
+  int rc = make_plan(cfg, B, T, &pl, true);
+  if (rc) return rc;
+  if ((int)sc->labels.size() != cfg->vocab_size) return fail(CTCDEC_E_INVALID, "scorer was built for %zu labels, decoder has %d", sc->labels.size(), cfg->vocab_size);
+  if ((rc = use_device(device))) return rc;
+  if (B == 0) return CTCDEC_OK;
+  std::lock_guard<std::mutex> lock(g_mu[device]);
+  DevCache &c = g_cache[device];
+  if (!c.stream) CU(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
+  cudaStream_t s = c.stream;
+  const int V = cfg->vocab_size, K = cfg->beam_size;
+  const size_t n_probs = (size_t)B * T * V, n_out = (size_t)B * K * T, n_bk = (size_t)B * K;
+  LmWorkspace w;
+  if ((rc = lm_workspace(sc, pl, B, &w))) return rc;
+  if ((rc = ensure(c, kBufInput, n_probs * 4 + 256))) return rc;
+  if ((rc = ensure(c, kBufTokens, n_out * 4 + 256))) return rc;
+  if ((rc = ensure(c, kBufTimesteps, n_out * 4 + 256))) return rc;
+  if ((rc = ensure(c, kBufSmall, small_bytes(B, K)))) return rc;
+  if ((rc = ensure(c, kBufWork, w.total + 256))) return rc;
+  float *d_probs = (float *)c.buf[kBufInput];
+  int *d_tok = (int *)c.buf[kBufTokens], *d_ts = (int *)c.buf[kBufTimesteps];
+  const SmallOut d = small_out(c.buf[kBufSmall], B, K);
+  LmBuffers io = lm_buffers(*sc, w, align256(c.buf[kBufWork]), PruneInput{d_probs, IN_F32, nullptr, true},
+                            DecodeOut{d_tok, d_ts, d.scores, d.lens, d.n_results, d.flags});
+  if (n_probs) CU(cudaMemcpyAsync(d_probs, probs, n_probs * 4, cudaMemcpyHostToDevice, s));
+  if (seq_lens) {
+    io.seq_lens = reinterpret_cast<int *>(io.ws + w.lens);
+    CU(cudaMemcpyAsync((int *)io.seq_lens, seq_lens, (size_t)B * 4, cudaMemcpyHostToDevice, s));
+  }
+  if ((rc = lm_batch_step(cfg, pl, sc, c, device, seq_lens, B, T, io, s))) return rc;
+  const bool lm_timing = getenv("CTCDEC_LM_TIMING") != nullptr;
+  const auto t_fin0 = std::chrono::steady_clock::now();
+  if ((rc = ensure_pinned(c, kPinSmall, small_bytes(B, K)))) return rc;
+  const SmallOut h = small_out(c.pin[kPinSmall], B, K);
+  if ((rc = read_small(h, d, K, 0, B, s))) return rc;
+  CU(cudaStreamSynchronize(s));
+  copy_result_rows(h, B, K, nullptr, scores, lens);
+  const int max_len = std::min(max_result_len(h, K, 0, B, nullptr), T);
+  if (max_len > 0) {
+    const size_t st_bytes = n_bk * (size_t)max_len * 8;
+    const bool staged = stage_rows(tokens, timesteps, st_bytes);
+    if (staged && (rc = ensure_pinned(c, kPinRows, st_bytes))) return rc;
+    int32_t *const stage_tok = staged ? static_cast<int32_t *>(c.pin[kPinRows]) : nullptr;
+    int32_t *const stage_ts = staged ? stage_tok + n_bk * (size_t)max_len : nullptr;
+    if ((rc = enqueue_rows(d_tok, d_ts, tokens, timesteps, stage_tok, stage_ts, n_bk, max_len, T, s))) return rc;
+    CU(cudaStreamSynchronize(s));
+    if (staged) spread_rows(stage_tok, stage_ts, tokens, timesteps, n_bk, max_len, T);
+  }
+  const auto t_fin1 = std::chrono::steady_clock::now();
+  lm_rescore_batch(*sc, B, K, T, h.n_results, tokens, lens, scores);  // reported scores: approx_ctc (reference :194-208)
+  if (lm_timing)
+    fprintf(stderr, "[ctcdec lm] finalize + copies back %.1f ms, read-out rescoring (sentence hook) %.1f ms, whole call %.1f ms\n",
+            std::chrono::duration<double>(t_fin1 - t_fin0).count() * 1e3,
+            std::chrono::duration<double>(std::chrono::steady_clock::now() - t_fin1).count() * 1e3,
+            std::chrono::duration<double>(std::chrono::steady_clock::now() - t_call0).count() * 1e3);
+  if (n_results) memcpy(n_results, h.n_results, (size_t)B * 4);
+  if (flags) memcpy(flags, h.flags, (size_t)B * 4);
+  return check_error_flags(h.flags, B);
 }
 
 // the checks both scorer device functions make before anything else: the scorer, the plan with a scorer, the labels
@@ -1899,31 +1921,40 @@ int ctcdec_lm_sweep_workspace_bytes(const ctcdec_config *cfg, const void *scorer
   return CTCDEC_OK;
 }
 
+// The checks the two device entries of the scorer path share once their plan is made, the current device, and the split
+// of the caller's workspace (which must hold `need` bytes) into *io.  B == 0 returns CTCDEC_OK before the workspace.
+static int lm_device_args(const HostScorer &sc, const LmWorkspace &w, const void *input, int kind, float *log_probs_out,
+                          int B, int T, const DecodeOut &o, void *workspace, size_t workspace_bytes, size_t need,
+                          int *device, LmBuffers *io) {
+  if (B > 0 && (!o.n_results || !o.flags)) return fail(CTCDEC_E_INVALID, "n_results and flags device buffers are required");
+  if (B > 0 && (!o.scores || !o.lens || (T > 0 && (!input || !o.tokens || !o.timesteps))))
+    return fail(CTCDEC_E_INVALID, "the input or an output pointer is NULL");
+  int rc = current_device(device);
+  if (rc || B == 0) return rc;
+  unsigned char *ws = nullptr;
+  if ((rc = workspace_start(workspace, workspace_bytes, need, &ws))) return rc;
+  *io = lm_buffers(sc, w, ws, PruneInput{input, kind, kind == IN_F32 ? nullptr : log_probs_out, true}, o);
+  return CTCDEC_OK;
+}
+
 int ctcdec_decode_batch_lm_device(const ctcdec_config *cfg, void *scorer, const void *input, int dtype,
                                   const int32_t *seq_lens, int B, int T, int32_t *tokens, int32_t *timesteps,
                                   float *scores, int32_t *lens, int32_t *n_results, int32_t *flags,
                                   float *log_probs_out, void *workspace, size_t workspace_bytes, void *stream) {
   if (!scorer) return fail(CTCDEC_E_INVALID, "scorer is NULL");
-  if (dtype != -1 && dtype != CTCDEC_DTYPE_F32 && dtype != CTCDEC_DTYPE_F16 && dtype != CTCDEC_DTYPE_BF16)
-    return fail(CTCDEC_E_INVALID, "dtype %d is not -1 (probabilities) or one of CTCDEC_DTYPE_F32 / F16 / BF16", dtype);
-  const int kind = dtype == -1 ? IN_F32 : dtype == CTCDEC_DTYPE_F32 ? IN_LOGITS_F32
-                 : dtype == CTCDEC_DTYPE_F16 ? IN_LOGITS_F16 : IN_LOGITS_BF16;
+  int kind = 0;
+  int rc = input_kind(dtype, true, &kind);
+  if (rc) return rc;
   Plan pl;
   LmWorkspace w;
-  int rc = lm_device_plan(cfg, scorer, B, T, &pl, &w);
-  if (rc) return rc;
+  if ((rc = lm_device_plan(cfg, scorer, B, T, &pl, &w))) return rc;
   HostScorer *sc = static_cast<HostScorer *>(scorer);
-  if (B > 0 && (!n_results || !flags)) return fail(CTCDEC_E_INVALID, "n_results and flags device buffers are required");
-  if (B > 0 && (!scores || !lens || (T > 0 && (!input || !tokens || !timesteps))))
-    return fail(CTCDEC_E_INVALID, "the input or an output pointer is NULL");
-  if ((rc = check_device())) return rc;
   int device = 0;
-  CU(cudaGetDevice(&device));
-  if (device >= 64) return fail(CTCDEC_E_INVALID, "device %d out of range", device);
-  if (B == 0) return CTCDEC_OK;
-  const size_t need_bytes = w.total + 256;
-  if (!workspace || workspace_bytes < need_bytes)
-    return fail(CTCDEC_E_WORKSPACE, "workspace of %zu bytes given, %zu needed", workspace_bytes, need_bytes);
+  LmBuffers io;
+  if ((rc = lm_device_args(*sc, w, input, kind, log_probs_out, B, T,
+                           DecodeOut{tokens, timesteps, scores, lens, n_results, flags}, workspace, workspace_bytes,
+                           w.total + 256, &device, &io)) || B == 0)
+    return rc;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   // the host answers the beam kernel's per-frame handshake while the call runs: a captured graph could not replay that
   cudaStreamCaptureStatus capturing = cudaStreamCaptureStatusNone;
@@ -1935,49 +1966,32 @@ int ctcdec_decode_batch_lm_device(const ctcdec_config *cfg, void *scorer, const 
   const size_t n_bk = (size_t)B * K;
   std::lock_guard<std::mutex> lock(g_mu[device]);
   DevCache &c = g_cache[device];
-  unsigned char *ws = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(workspace) + 255) / 256 * 256);
-  int *d_lens_in = seq_lens ? reinterpret_cast<int *>(ws + w.lens) : nullptr;
-  if (seq_lens) CU(cudaMemcpyAsync(d_lens_in, seq_lens, (size_t)B * 4, cudaMemcpyHostToDevice, s));
-  LmBuffers io;
-  io.in = PruneInput{input, kind, kind == IN_F32 ? nullptr : log_probs_out, true};
-  io.seq_lens = d_lens_in;
-  io.ws = ws;
-  io.lm_arena = reinterpret_cast<float *>(ws + w.lm_arena);
-  io.dstate = reinterpret_cast<int *>(ws + w.dstate);
-  io.lm_row = sc->is_character_based ? reinterpret_cast<float *>(ws + w.rows) : nullptr;
-  io.lm_hist = sc->ngram ? reinterpret_cast<int *>(ws + w.hist) : nullptr;
-  io.tokens = tokens; io.timesteps = timesteps; io.scores = scores; io.lens = lens; io.n_results = n_results;
-  io.flags = flags;
+  if (seq_lens) {
+    io.seq_lens = reinterpret_cast<int *>(io.ws + w.lens);
+    CU(cudaMemcpyAsync((int *)io.seq_lens, seq_lens, (size_t)B * 4, cudaMemcpyHostToDevice, s));
+  }
   if ((rc = lm_batch_step(cfg, pl, sc, c, device, seq_lens, B, T, io, s))) return rc;
   // Read-out: the finalize kernel wrote the rows in place; the reported scores are the reference's approx_ctc, which
   // needs the sentence hook on each row's labels, so columns [0, max_len) of the rows come to pinned staging
-  std::unique_ptr<int[]> h_nres(new int[(size_t)B * 2]);
-  int *const h_flags = h_nres.get() + B;
-  std::unique_ptr<float[]> h_scores(new float[n_bk]);
-  std::unique_ptr<int[]> h_lens(new int[n_bk]);
-  CU(cudaMemcpyAsync(h_scores.get(), scores, n_bk * 4, cudaMemcpyDeviceToHost, s));
-  CU(cudaMemcpyAsync(h_lens.get(), lens, n_bk * 4, cudaMemcpyDeviceToHost, s));
-  CU(cudaMemcpyAsync(h_nres.get(), n_results, (size_t)B * 4, cudaMemcpyDeviceToHost, s));
-  CU(cudaMemcpyAsync(h_flags, flags, (size_t)B * 4, cudaMemcpyDeviceToHost, s));
+  if ((rc = ensure_pinned(c, kPinSmall, small_bytes(B, K)))) return rc;
+  const SmallOut h = small_out(c.pin[kPinSmall], B, K);
+  if ((rc = read_small(h, SmallOut{scores, lens, n_results, flags}, K, 0, B, s))) return rc;
   CU(cudaStreamSynchronize(s));
-  int max_len = 0;
-  for (int b = 0; b < B; ++b)
-    for (int p = 0; p < h_nres[b] && p < K; ++p) max_len = std::max(max_len, h_lens[(size_t)b * K + p]);
-  if (max_len > T) max_len = T;
+  const int max_len = std::min(max_result_len(h, K, 0, B, nullptr), T);
   static const int32_t no_rows = 0;
   const int32_t *stage_tok = &no_rows;
   if (max_len > 0) {
-    if ((rc = ensure_pinned(c, 5, n_bk * (size_t)max_len * 4))) return rc;
-    int32_t *const st = static_cast<int32_t *>(c.pin[5]);
+    if ((rc = ensure_pinned(c, kPinRows, n_bk * (size_t)max_len * 4))) return rc;
+    int32_t *const st = static_cast<int32_t *>(c.pin[kPinRows]);
     CU(cudaMemcpy2DAsync(st, (size_t)max_len * 4, tokens, (size_t)T * 4, (size_t)max_len * 4, n_bk, cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
     stage_tok = st;
   }
-  lm_rescore_batch(*sc, B, K, max_len, h_nres.get(), stage_tok, h_lens.get(), h_scores.get());
+  lm_rescore_batch(*sc, B, K, max_len, h.n_results, stage_tok, h.lens, h.scores);
   // (rows p >= n_results[b] go back as they were read: the caller's values, unchanged)
-  CU(cudaMemcpyAsync(scores, h_scores.get(), n_bk * 4, cudaMemcpyHostToDevice, s));
+  CU(cudaMemcpyAsync(scores, h.scores, n_bk * 4, cudaMemcpyHostToDevice, s));
   CU(cudaStreamSynchronize(s));
-  return check_error_flags(h_flags, B);
+  return check_error_flags(h.flags, B);
 }
 
 // ctcdec_decode_batch_lm_device_async (P = 0: the scorer's alpha and beta) and ctcdec_decode_batch_lm_sweep_async (P >= 1
@@ -1987,15 +2001,14 @@ static int lm_decode_async(const ctcdec_config *cfg, void *scorer, const void *i
                            int32_t *tokens, int32_t *timesteps, float *scores, int32_t *lens, int32_t *n_results,
                            int32_t *flags, float *log_probs_out, void *workspace, size_t workspace_bytes, void *stream) {
   if (!scorer) return fail(CTCDEC_E_INVALID, "scorer is NULL");
-  if (dtype != -1 && dtype != CTCDEC_DTYPE_F32 && dtype != CTCDEC_DTYPE_F16 && dtype != CTCDEC_DTYPE_BF16)
-    return fail(CTCDEC_E_INVALID, "dtype %d is not -1 (probabilities) or one of CTCDEC_DTYPE_F32 / F16 / BF16", dtype);
-  const int kind = dtype == -1 ? IN_F32 : dtype == CTCDEC_DTYPE_F32 ? IN_LOGITS_F32
-                 : dtype == CTCDEC_DTYPE_F16 ? IN_LOGITS_F16 : IN_LOGITS_BF16;
+  int kind = 0;
+  int rc = input_kind(dtype, true, &kind);
+  if (rc) return rc;
   const bool sweep = P > 0;
   Plan pl;
   LmWorkspace w;
   size_t need_bytes = 0;
-  int rc = sweep ? lm_sweep_plan(cfg, scorer, B, T, P, &pl, &w, &need_bytes) : lm_device_plan(cfg, scorer, B, T, &pl, &w);
+  rc = sweep ? lm_sweep_plan(cfg, scorer, B, T, P, &pl, &w, &need_bytes) : lm_device_plan(cfg, scorer, B, T, &pl, &w);
   if (rc) return rc;
   if (!sweep) need_bytes = w.total + 256;
   HostScorer *sc = static_cast<HostScorer *>(scorer);
@@ -2003,16 +2016,12 @@ static int lm_decode_async(const ctcdec_config *cfg, void *scorer, const void *i
     return fail(CTCDEC_E_UNSUPPORTED, "the asynchronous scorer decode takes a scorer from ctcdec_scorer_create_arpa only: "
                 "a hook scorer needs the host during the call (use ctcdec_decode_batch_lm_device)");
   if (sweep && (!alphas || !betas)) return fail(CTCDEC_E_INVALID, "alphas and betas (host double[P]) are required");
-  if (B > 0 && (!n_results || !flags)) return fail(CTCDEC_E_INVALID, "n_results and flags device buffers are required");
-  if (B > 0 && (!scores || !lens || (T > 0 && (!input || !tokens || !timesteps))))
-    return fail(CTCDEC_E_INVALID, "the input or an output pointer is NULL");
-  if ((rc = check_device())) return rc;
   int device = 0;
-  CU(cudaGetDevice(&device));
-  if (device >= 64) return fail(CTCDEC_E_INVALID, "device %d out of range", device);
-  if (B == 0) return CTCDEC_OK;
-  if (!workspace || workspace_bytes < need_bytes)
-    return fail(CTCDEC_E_WORKSPACE, "workspace of %zu bytes given, %zu needed", workspace_bytes, need_bytes);
+  LmBuffers io;
+  if ((rc = lm_device_args(*sc, w, input, kind, log_probs_out, B, T,
+                           DecodeOut{tokens, timesteps, scores, lens, n_results, flags}, workspace, workspace_bytes,
+                           need_bytes, &device, &io)) || B == 0)
+    return rc;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   cudaStreamCaptureStatus capturing = cudaStreamCaptureStatusNone;
   CU(cudaStreamIsCapturing(s, &capturing));
@@ -2026,20 +2035,10 @@ static int lm_decode_async(const ctcdec_config *cfg, void *scorer, const void *i
     explicit CaptureGuard(bool on) { g_capturing = on; }
     ~CaptureGuard() { g_capturing = false; }
   } guard(capturing != cudaStreamCaptureStatusNone);
-  unsigned char *ws = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(workspace) + 255) / 256 * 256);
-  LmBuffers io;
-  io.in = PruneInput{input, kind, kind == IN_F32 ? nullptr : log_probs_out, true};
   io.seq_lens = seq_lens;
-  io.ws = ws;
-  io.lm_arena = reinterpret_cast<float *>(ws + w.lm_arena);
-  io.dstate = reinterpret_cast<int *>(ws + w.dstate);
-  io.lm_row = sc->is_character_based ? reinterpret_cast<float *>(ws + w.rows) : nullptr;
-  io.lm_hist = reinterpret_cast<int *>(ws + w.hist);
-  io.tokens = tokens; io.timesteps = timesteps; io.scores = scores; io.lens = lens; io.n_results = n_results;
-  io.flags = flags;
   if (sweep) {
     // each pair through float32, as ctcdec_scorer_reset_params stores them
-    double *tab = reinterpret_cast<double *>(ws + w.total);
+    double *tab = reinterpret_cast<double *>(io.ws + w.total);
     for (int p0 = 0; p0 < P; p0 += kTabPerLaunch) {
       SweepPairArgs a;
       a.tab = tab; a.p0 = p0; a.n = std::min(kTabPerLaunch, P - p0);
@@ -2099,9 +2098,7 @@ int ctcdec_scorer_rescore_rows(void *scorer, const int32_t *tokens, const int32_
     return CTCDEC_OK;
   }
   if (!sc->ngram) return fail(CTCDEC_E_UNSUPPORTED, "the read-out kernel takes a scorer from ctcdec_scorer_create_arpa only");
-  if (device >= 64) return fail(CTCDEC_E_INVALID, "device %d out of range", device);
-  if (cudaSetDevice(device) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "cudaSetDevice(%d) failed", device);
-  int rc = check_device();
+  int rc = use_device(device);
   if (rc) return rc;
   if (B == 0) return CTCDEC_OK;
   std::lock_guard<std::mutex> lock(g_mu[device]);
@@ -2138,8 +2135,7 @@ int ctcdec_rows_to_host(const int32_t *d_tokens, const int32_t *d_timesteps, lon
 
 int ctcdec_selftest_math_f64(int which, const double *x, const double *x2, double *y, size_t n, int device) {
   if (which < 0 || which > 2 || !x || !y || (which == 2 && !x2)) return fail(CTCDEC_E_INVALID, "bad selftest arguments");
-  if (cudaSetDevice(device) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "cudaSetDevice(%d) failed", device);
-  int rc = check_device();
+  int rc = use_device(device);
   if (rc) return rc;
   if (n == 0) return CTCDEC_OK;
   double *dx = nullptr, *dx2 = nullptr, *dy = nullptr;
@@ -2158,8 +2154,7 @@ int ctcdec_selftest_math_f64(int which, const double *x, const double *x2, doubl
 
 int ctcdec_selftest_math(int which, const float *x, const float *x2, float *y, size_t n, int device) {
   if (which < 0 || which > 3 || !x || !y || (which == 3 && !x2)) return fail(CTCDEC_E_INVALID, "bad selftest arguments");
-  if (cudaSetDevice(device) != cudaSuccess) return fail(CTCDEC_E_NO_DEVICE, "cudaSetDevice(%d) failed", device);
-  int rc = check_device();
+  int rc = use_device(device);
   if (rc) return rc;
   if (n == 0) return CTCDEC_OK;
   float *dx = nullptr, *dx2 = nullptr, *dy = nullptr;
