@@ -2,6 +2,10 @@
 // Included by ctc_kernels.cu (device build) and tests/native/emulate_cta.cpp (CTC_EMULATE, test only).
 #pragma once
 #include "beam_core.cuh"
+#if defined(CTC_EMULATE)
+#include <cstdio>   // (the emulation's histogram check)
+#include <cstdlib>
+#endif
 
 // compile-time switches of the barrier-free back half (tools/build_variants.sh builds A/B variants with -D...).
 // The frame loop is bound by its INSTRUCTION FOOTPRINT: each of these features is a win on paper but adds code to the
@@ -78,6 +82,22 @@ static EmuStats g_stats;
 #define CTC_STAT(x) (x)
 #else
 #define CTC_STAT(x) ((void)0)
+#endif
+
+// one count into a radix histogram of kNBins ints.  A key outside the range the bins were laid over would index past
+// the histogram -- on the device an out-of-bounds shared-memory atomic -- so the CPU emulation checks every bin and
+// stops the decode with a message.
+#if defined(CTC_EMULATE)
+static inline void emu_hist_add(int *hist, unsigned long long bin, const char *file, int line) {
+  if (bin >= (unsigned long long)kNBins) {
+    fprintf(stderr, "%s:%d: radix histogram bin %llu out of range [0, %d)\n", file, line, bin, kNBins);
+    abort();
+  }
+  ++hist[bin];
+}
+#define CTC_HIST_ADD(hist, bin) emu_hist_add((hist), (bin), __FILE__, __LINE__)
+#else
+#define CTC_HIST_ADD(hist, bin) atom_add(&(hist)[(int)(bin)], 1)
 #endif
 
 #if defined(CTC_EMULATE)
@@ -733,6 +753,9 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
         lpm = lpb > lpm ? lpb : lpm;
       }
       top = ord_f(f_add(f_add(cmax, lpm), 1.5f));
+      // (a frame that keeps no character at all, cutoff_top_n = 0: -FLT_MAX + -FLT_MAX rounds to -inf, below the
+      // members' -FLT_MAX scores)
+      if (top < ord_f(kNInf)) top = ord_f(kNInf);
       lov = lo;
       if (full && !p.force_fallback) {
         // A second, usually much tighter bound (where the vocabulary is cut per frame the blank is often not among
@@ -857,13 +880,29 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
           const unsigned o = ord_f(sn);
           if (!LM) {
             // first radix pass: the member bins itself (the histograms were cleared by region R5)
-            if (o >= lo32) atom_add(&hist0[(int)((o - lo32) >> shift32)], 1);
+            if (o >= lo32) CTC_HIST_ADD(hist0, (o - lo32) >> shift32);
           } else {
             kmin = o < kmin ? o : kmin;
             kmax = o > kmax ? o : kmax;
-            const unsigned os = ord_f(sc);
-            smax = os > smax ? os : smax;
           }
+        }
+      }
+      if (LM) {
+        // the largest key each member's grid row can reach before beta: its score + the frame's best non-blank
+        // log-prob + the row's largest LM term when that is positive (alpha < 0, or a backoff weight > 0).  (A loop
+        // of its own: inside the one above it costs the index-order scorer kernel a spill.)
+        for (int j = tid; j < M; j += NT) {
+          float tm = 0.0f;
+          if (!c.lm_char) {
+            tm = c.s_lmsp[j] > tm ? c.s_lmsp[j] : tm;
+          } else {
+            const float *const row = c.lm_row + (size_t)c.s_node[j] * V;
+            for (int r = 0; r < n; ++r) { const float x = ld_cg(&row[c.chr_at(r)]); tm = x > tm ? x : tm; }
+          }
+          float u = f_add(c.s_score[j], lpmax);
+          if (tm > 0.0f) u = f_add(u, tm);
+          const unsigned os = ord_f(u);
+          smax = os > smax ? os : smax;
         }
       }
       if (npairs) atom_add(&s_ctl[MERGED ? npairs_w : (int)C_NPAIRS], npairs);
@@ -880,7 +919,8 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
           }
         }
       }
-      if (LM) {  // with a scorer the range is taken from the new member scores (the LM term is not bounded above)
+      if (LM) {  // with a scorer the range is taken from the new member scores and the rows' bounds (the LM term is not
+                 // bounded above)
 #if defined(CTC_EMULATE)
         red_min_u32((unsigned *)&s_ctl[C_KMIN], kmin);
         red_max_u32((unsigned *)&s_ctl[C_KMAX], kmax);
@@ -918,7 +958,7 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
         CTC_LANES {
           for (int j = warp * 32 + lane; j < M; j += NT) {
             const unsigned k = ord_f(c.s_snew[j]);
-            if (k >= lo32) atom_add(&hist0[(int)((k - lo32) >> shift32)], 1);
+            if (k >= lo32) CTC_HIST_ADD(hist0, (k - lo32) >> shift32);
           }
         }
       }
@@ -973,7 +1013,7 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
               const bool ok = !((c.s_mask[i * WS + (mb >> 5)] >> (mb & 31)) & 1u) && (k >= lo32);
               pred[LX] = ok ? 1 : 0;
               kk[LX] = k;
-              if (ok && !select_all) atom_add(&hist0[(int)((k - lo32) >> shift32)], 1);
+              if (ok && !select_all) CTC_HIST_ADD(hist0, (k - lo32) >> shift32);
             }
           }
           const unsigned bal = ctc_ballot(pred);
@@ -1044,8 +1084,8 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
             pred1[LX] = ok1 ? 1 : 0; kk1[LX] = k1;
             pred2[LX] = ok2 ? 1 : 0; kk2[LX] = k2;
             if (!select_all) {
-              if (ok1) atom_add(&hist0[(int)((k1 - lo32) >> shift32)], 1);
-              if (ok2) atom_add(&hist0[(int)((k2 - lo32) >> shift32)], 1);
+              if (ok1) CTC_HIST_ADD(hist0, (k1 - lo32) >> shift32);
+              if (ok2) CTC_HIST_ADD(hist0, (k2 - lo32) >> shift32);
             }
           }
           const unsigned bal1 = ctc_ballot(pred1), bal2 = ctc_ballot(pred2);
@@ -1100,8 +1140,8 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
               pred1[LX] = ok1 ? 1 : 0; kk1[LX] = k1;
               pred2[LX] = ok2 ? 1 : 0; kk2[LX] = k2;
               if (!select_all) {
-                if (ok1) atom_add(&hist0[(int)((k1 - lo32) >> shift32)], 1);
-                if (ok2) atom_add(&hist0[(int)((k2 - lo32) >> shift32)], 1);
+                if (ok1) CTC_HIST_ADD(hist0, (k1 - lo32) >> shift32);
+                if (ok2) CTC_HIST_ADD(hist0, (k2 - lo32) >> shift32);
               }
             }
             const unsigned bal1 = ctc_ballot(pred1), bal2 = ctc_ballot(pred2);
@@ -1160,8 +1200,8 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
               pred1[LX] = ok1 ? 1 : 0; kk1[LX] = k1;
               pred2[LX] = ok2 ? 1 : 0; kk2[LX] = k2;
               if (!select_all) {
-                if (ok1) atom_add(&hist0[(int)((k1 - lo32) >> shift32)], 1);
-                if (ok2) atom_add(&hist0[(int)((k2 - lo32) >> shift32)], 1);
+                if (ok1) CTC_HIST_ADD(hist0, (k1 - lo32) >> shift32);
+                if (ok2) CTC_HIST_ADD(hist0, (k2 - lo32) >> shift32);
               }
             }
             const unsigned bal1 = ctc_ballot(pred1), bal2 = ctc_ballot(pred2);
@@ -1216,7 +1256,7 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
               const bool ok = (ch >= 0) && !mk && (k >= lo32) && okl;
               pred[LX] = ok ? 1 : 0;
               kk[LX] = k;
-              if (ok && !select_all) atom_add(&hist0[(int)((k - lo32) >> shift32)], 1);
+              if (ok && !select_all) CTC_HIST_ADD(hist0, (k - lo32) >> shift32);
             }
             const unsigned bal = ctc_ballot(pred);
             if (bal) {
@@ -1249,10 +1289,11 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
       if (LM) {
         lo32 = (!select_all && M == K) ? (unsigned)s_ctl[C_KMIN] : 0u;
         top32 = (unsigned)s_ctl[C_KMAX];
-        // a scored candidate gains its LM term (<= 0) and beta: with beta > 0 it can end above the best member score
-        // plus the row's best log-prob, by at most beta (its key outside the range would index past the histogram)
+        // a scored candidate gains its LM term and beta, either of which can be positive: its key is at most its row's
+        // bound from region R1 (score + best log-prob + the row's largest positive term) plus max(0, beta).  Every
+        // step rounds monotonically, so no key the grid walk bins lies above top32 (it would index past the histogram).
         const double bmax = c.s_ab[1] > 0.0 ? c.s_ab[1] : 0.0;
-        const unsigned o = ord_f((float)d_add((double)f_add(unord_f((unsigned)s_ctl[C_SMAX]), lpmax), bmax));
+        const unsigned o = ord_f((float)d_add((double)unord_f((unsigned)s_ctl[C_SMAX]), bmax));
         top32 = o > top32 ? o : top32;
         set_shift();
       }
@@ -1285,7 +1326,7 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
             if (!select_all)
               for (int j = tid; j < M; j += NT) {
                 const unsigned k = ord_f(c.s_snew[j]);
-                if (k >= lo32) atom_add(&hist0[(int)((k - lo32) >> shift32)], 1);
+                if (k >= lo32) CTC_HIST_ADD(hist0, (k - lo32) >> shift32);
               }
           }
         }
