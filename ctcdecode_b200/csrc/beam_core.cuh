@@ -237,6 +237,7 @@ struct BeamParams {
   int no_fast;              // test knob: never take the barrier-free back half of a frame
   float heur_bias;          // test knob: added to the checked heuristic bound (> 0 makes it fail its check often)
   const unsigned char *finalize;  // [B] or nullptr (= finalize all)
+  int backtrace;          // 1: an index-order kernel without a scorer runs finalize_cta_run after its last frame itself
   int *out_tokens, *out_timesteps;  // [B][K][out_T]
   float *out_scores;                // [B][K]
   int *out_lens;                    // [B][K]

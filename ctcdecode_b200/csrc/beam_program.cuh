@@ -347,6 +347,9 @@ CTC_FN void flush_lpc_ts(Node *p, float lpc, int ts) {
 #endif
 }
 
+template <int NT>
+CTC_FN void finalize_cta_run(const BeamParams &p, const int b, unsigned char *smem);
+
 // ======================================================================================================
 //  beam_cta_run: consume frames [0, Tb) of utterance b, leave the beam state in global memory.
 // ======================================================================================================
@@ -1908,6 +1911,13 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
       p.timing[(size_t)gridDim.x * 16 + (size_t)b * 16 * 32 + x] = s_wbusy[x];
   }
 #endif
+  if (MERGED && p.backtrace) {
+    // the backtrace of this utterance, by this CTA, while other CTAs still run their frames: no finalize launch, and
+    // only the last CTA's backtrace is left exposed.  It reads the state block stored above and takes the slot block
+    // of shared memory (the head keeps the tile barriers and the timing counters; the host checks the size).
+    CTC_BARRIER();
+    finalize_cta_run<NT>(p, b, smem + kSmemHead);
+  }
 }
 
 // ======================================================================================================
@@ -1929,6 +1939,11 @@ CTC_HD int finalize_rounds_cap(int K) {  // checkpoints per prefix and round: wh
 CTC_HD size_t finalize_smem_bytes(int K) {
   // keys [K] u64, order [K], flag, cur node [K], cur depth [K], checkpoint count [K], checkpoints [K][R]
   return (size_t)K * 8 + (size_t)K * 4 * 4 + (size_t)K * finalize_rounds_cap(K) * 4 + 64;
+}
+// Does a one-launch offline decode run the backtrace in the beam kernel's epilogue (BeamParams::backtrace)?  Index-order
+// kernels without a scorer do, in the shared memory behind the layout's head (the slot block alone is larger).
+CTC_HD bool cta_backtrace(bool sorted, int K, const SmemLayout &L) {
+  return !sorted && kSmemHead + finalize_smem_bytes(K) <= (size_t)L.total;
 }
 template <int NT>
 CTC_FN void finalize_cta_run(const BeamParams &p, const int b, unsigned char *smem) {
@@ -2000,23 +2015,38 @@ CTC_FN void finalize_cta_run(const BeamParams &p, const int b, unsigned char *sm
       }
     }
     CTC_BARRIER();
-    // (b) every (prefix, checkpoint) pair: the stretch of at most kJump nodes below the checkpoint's jump target
+    // (b) every (prefix, checkpoint) pair: the stretch of at most kJump nodes below the checkpoint's jump target.
+    // Each thread walks U stretches in lockstep, so that a CTA of fewer than 1024 threads (the beam kernel's own
+    // backtrace) keeps as many independent hops in flight as the 1024-thread finalize kernel.
+    constexpr int U = NT >= 1024 ? 1 : 1024 / NT;
     CTC_PAR {
-      for (int it = tid; it < M * R; it += NT) {
-        const int q = it / R, k = it - q * R;
-        if (k >= s_ncp[q]) continue;
-        const int d0 = s_dep[q];
-        int d = (k == 0) ? d0 : ((d0 - 1) / kJump) * kJump - (k - 1) * kJump;  // depth of the k-th checkpoint
-        const int dend = ((d - 1) / kJump) * kJump;
-        int nid = s_cp[(size_t)q * R + k];
-        const size_t row = ((size_t)b * K + q) * (size_t)p.out_T;
-        for (; d > dend; --d) {
-          const Node nd = load_node(&nodes[nid]);
-          if (d - 1 < p.out_T) {
-            p.out_tokens[row + d - 1] = nd.chr;
-            p.out_timesteps[row + d - 1] = nd.ts;
+      for (int it0 = tid; it0 < M * R; it0 += U * NT) {
+        int nid[U], d[U], dend[U];
+        size_t row[U];
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          const int it = it0 + u * NT;
+          const int q = it / R, k = it - q * R;
+          d[u] = 0; dend[u] = 0; nid[u] = 0; row[u] = 0;
+          if (it >= M * R || k >= s_ncp[q]) continue;
+          const int d0 = s_dep[q];
+          d[u] = (k == 0) ? d0 : ((d0 - 1) / kJump) * kJump - (k - 1) * kJump;  // depth of the k-th checkpoint
+          dend[u] = ((d[u] - 1) / kJump) * kJump;
+          nid[u] = s_cp[(size_t)q * R + k];
+          row[u] = ((size_t)b * K + q) * (size_t)p.out_T;
+        }
+        for (int h = 0; h < kJump; ++h) {
+#pragma unroll
+          for (int u = 0; u < U; ++u) {
+            if (d[u] <= dend[u]) continue;
+            const Node nd = load_node(&nodes[nid[u]]);
+            if (d[u] - 1 < p.out_T) {
+              p.out_tokens[row[u] + d[u] - 1] = nd.chr;
+              p.out_timesteps[row[u] + d[u] - 1] = nd.ts;
+            }
+            nid[u] = nd.parent;
+            --d[u];
           }
-          nid = nd.parent;
         }
       }
     }

@@ -454,6 +454,7 @@ static int ensure(DevCache &c, int slot, size_t bytes) {
 struct Profile {
   bool on = false;
   bool valid = false;
+  bool fused_finalize = false;  // the beam kernel ran the backtrace itself: ev[2] and ev[3] bracket no kernel
   long long *timing = nullptr;  // device buffer [B][16] for per-region cycle counts (diagnostic)
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
 };
@@ -912,12 +913,14 @@ static int decode_device_impl(const ctcdec_config *cfg, const PruneInput &in, co
   BeamParams bp = beam_params(*cfg, pl, ws, seq_lens, T, DecodeOut{tokens, timesteps, scores, lens, n_results, flags}, T);
   flat_arenas(bp, pl, ws);
   bp.tile_frames = pl.F; bp.fresh = 1;
+  bp.backtrace = cta_backtrace(pl.sorted, bp.K, pl.L);
   if ((rc = launch_beam(bp, pl, B, s))) return rc;
   if (prof) CU(cudaEventRecord(g_prof.ev[2], s));
-  if ((rc = launch_finalize(bp, B, s))) return rc;
+  if (!bp.backtrace && (rc = launch_finalize(bp, B, s))) return rc;
   if (prof) {
     CU(cudaEventRecord(g_prof.ev[3], s));
     g_prof.valid = true;
+    g_prof.fused_finalize = bp.backtrace != 0;
   }
   return CTCDEC_OK;
 }
@@ -980,6 +983,7 @@ int ctcdec_profile_read(float *ms) {
   if (!g_prof.valid) return fail(CTCDEC_E_INVALID, "no profiled decode on this thread");
   CU(cudaEventSynchronize(g_prof.ev[3]));
   for (int i = 0; i < 3; ++i) CU(cudaEventElapsedTime(&ms[i], g_prof.ev[i], g_prof.ev[i + 1]));
+  if (g_prof.fused_finalize) ms[2] = 0.0f;
   return CTCDEC_OK;
 }
 

@@ -396,8 +396,10 @@ int ctcdec_stream_committed_device(void *const *states, int B, const int32_t *si
 
 /* ---- measurement hook (bench.py) --------------------------------------------------------------------
  * With profiling enabled on the calling thread, ctcdec_decode_batch_device records CUDA events on its stream
- * around each of its three kernels; ctcdec_profile_read waits for the last decode of this thread and returns
- * the device time in milliseconds of {prune/log scan, beam search, finalize}. */
+ * around each of its kernels; ctcdec_profile_read waits for the last decode of this thread and returns
+ * the device time in milliseconds of {prune/log scan, beam search, finalize}.  When nothing is cut from the
+ * vocabulary (cutoff_prob = 1 and cutoff_top_n >= vocab_size) the beam kernel runs the backtrace itself: there
+ * is no finalize kernel, its time is reported as 0, and the beam search time includes the backtrace. */
 int ctcdec_profile_enable(int on);
 int ctcdec_profile_read(float *ms3);
 /* Diagnostic: if device_buffer (int64 [B][16] followed by int64 [B][16][32], device memory) is non-NULL, every
