@@ -70,6 +70,11 @@ _SIGNATURES = {
     "ctcdec_decode_batch_lm_sweep_async": (ctypes.c_int, [ctypes.POINTER(Config), _vp, _vp, ctypes.c_int, _vp,
                                                           ctypes.c_int, ctypes.c_int, _vp, _vp, ctypes.c_int, _vp, _vp,
                                                           _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_size_t, _vp]),
+    "ctcdec_lm_mixed_workspace_bytes": (ctypes.c_int, [ctypes.POINTER(Config), ctypes.POINTER(_vp), ctypes.c_int,
+                                                       ctypes.c_int, ctypes.c_int, ctypes.POINTER(ctypes.c_size_t)]),
+    "ctcdec_decode_batch_lm_mixed_async": (ctypes.c_int, [ctypes.POINTER(Config), ctypes.POINTER(_vp), ctypes.c_int,
+                                                          _vp, _vp, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int, _vp,
+                                                          _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_size_t, _vp]),
     "ctcdec_scorer_rescore_rows": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.c_int,
                                                   ctypes.c_int]),
     "ctcdec_state_create":(ctypes.c_int, [ctypes.POINTER(Config), ctypes.c_int, ctypes.POINTER(_vp)]),
@@ -78,6 +83,8 @@ _SIGNATURES = {
     "ctcdec_state_frames": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_int)]),
     "ctcdec_decode_stream_host": (ctypes.c_int, [_vp, _vp, ctypes.c_int, ctypes.c_int, ctypes.POINTER(_vp), _vp,
                                                  _vp, _vp, ctypes.c_int, _vp, _vp, _vp, _vp]),
+    "ctcdec_stream_states_workspace_bytes": (ctypes.c_int, [ctypes.POINTER(_vp), ctypes.c_int, ctypes.c_int,
+                                                            ctypes.POINTER(ctypes.c_size_t)]),
     "ctcdec_stream_workspace_bytes": (ctypes.c_int, [ctypes.POINTER(Config), ctypes.c_int, ctypes.c_int,
                                                      ctypes.POINTER(ctypes.c_size_t)]),
     "ctcdec_decode_stream_device": (ctypes.c_int, [_vp, ctypes.c_int, _vp, ctypes.c_int, ctypes.c_int,

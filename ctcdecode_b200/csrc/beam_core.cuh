@@ -216,7 +216,26 @@ CTC_HD SmemLayout make_layout(int K, int V, int NP, int tile_frames, bool sorted
   return L;
 }
 
-struct BeamParams {
+// One language model of a scorer decode, with its weights: the LM slot a beam CTA decodes with.  BeamParams derives from
+// it (after BeamCommon), so these fields of the kernel parameters are the call's model; a decode over several models (or weights) gives
+// each CTA a slot of BeamParams::lm_slots instead (beam_program.cuh, lm_slot).  Everything else of the scorer path
+// (space_id, dict_wc, lm_char) is call-wide.
+struct LmSlot {
+  const int *dict_next;             // [n_states][V]: -1 = no arc, else next state | kDictFinal | kDictSpace
+  const uint32_t *dict_mask;        // [n_states][dict_wc]: bit c = the state has an arc for character c
+  int dict_start;
+  double beta;                      // Scorer::beta
+  double lm_alpha;                  // Scorer::alpha: a term is float(cond_log_prob * alpha), as the host computes it
+  // device n-gram scorer only
+  NgramView ngram;                  // the model's tables in device memory
+  const int *word_of_state;         // word-based: [n_states] the word a dictionary state completes with a space
+  const int *label_word;            // character-based: [V] the word id of each label
+  int lm_hist_n;                    // order - 1
+  NgramFront front;                 // the read-out's front-end tables (labels' bytes, unigram spellings)
+};
+
+// The kernel parameters every decode has, at the start of BeamParams (the kernels without a scorer read nothing else).
+struct BeamCommon {
   const float *lp;        // [B][T][NP] pruned float32 log-probs from the prune kernel
   const uint16_t *idx;    // [B][T][NP] character of each pruned entry, 0xFFFF = unused (sorted mode only)
   const int *seq_lens;    // [B] or nullptr
@@ -245,15 +264,15 @@ struct BeamParams {
   int out_T;
   int *flags;  // [B], OR-ed
   long long *timing;  // optional [B][16]: cycles thread 0 spent between consecutive barriers, per region
+};
+
+struct BeamParams : BeamCommon, LmSlot {
   // ---- scorer path (word-based LM + dictionary, reference ctc_beam_search_decoder.cpp:74-82,93-95,120-137 and
-  //      path_trie.cpp:59-96); everything below is unused (0 / nullptr) when no scorer is attached
-  const int *dict_next;             // [n_states][V]: -1 = no arc, else next state | kDictFinal | kDictSpace
-  const uint32_t *dict_mask;        // [n_states][dict_wc]: bit c = the state has an arc for character c
+  //      path_trie.cpp:59-96); everything below, and the LmSlot fields, are unused (0 / nullptr) when no scorer is
+  //      attached
   int dict_wc;                      // words per mask row, ceil(V / 32)
-  int dict_start;
   int space_id;                     // label of " ", -2 if there is none (reference :34-40)
-  double beta;                      // Scorer::beta
-  float *lm_arena;                  // [B][arena_stride]: per node float(cond_log_prob(make_ngram(node)) * alpha)
+  float *lm_arena;                 // [B][arena_stride]: per node float(cond_log_prob(make_ngram(node)) * alpha)
   int *dstate_arena;                // [B][arena_stride]: per node dictionary state
   // The exchange with the host's Scorer hook: two blocks per utterance in device-mapped pinned host memory, each
   // starting on its own 128-byte line (lm_nl_stride / lm_up_stride ints apart, lm_host.h exchange_strides):
@@ -283,17 +302,21 @@ struct BeamParams {
   // device n-gram scorer (an ARPA scorer, ngram_lm.h): the CTA computes the LM terms of the nodes it creates itself, so
   // there are no exchange blocks and no handshake (lm_persistent = 0, newlist / lm_upd unused)
   int lm_dev;
-  double lm_alpha;                  // Scorer::alpha: a term is float(cond_log_prob * alpha), as the host computes it
-  NgramView ngram;                  // the model's tables in device memory
-  const int *word_of_state;         // word-based: [n_states] the word a dictionary state completes with a space
-  const int *label_word;            // character-based: [V] the word id of each label
-  int lm_hist_n;                    // order - 1
-  int *lm_hist;                     // [B][arena_stride][order - 1] the node's last order - 1 LM word ids, oldest first
-  // sweep of the LM weights (ctcdec_decode_batch_lm_sweep_async): CTA g decodes input row g % sweep_B (lp, idx,
-  // seq_lens) with the pair lm_ab[g / sweep_B] = (alpha, beta) in place of lm_alpha / beta; everything else is indexed
-  // by g.  sweep_B = 0 (and lm_ab = NULL): CTA g decodes row g with lm_alpha / beta.
+  int *lm_hist;                     // [B][arena_stride][lm_hist_stride] the node's last order - 1 LM word ids, oldest first
+  // Per-CTA LM slots.  CTA g's slot index is s = lm_slot_of[g], or g / sweep_B without lm_slot_of (0 without either).
+  // Its model and weights are lm_slots[s] (or the call's, the LmSlot fields above, without lm_slots), except that
+  // lm_ab[s] = (alpha, beta) replaces the weights when lm_ab is set.
+  //   sweep of the LM weights (ctcdec_decode_batch_lm_sweep_async): CTA g decodes input row g % sweep_B (lp, idx,
+  //     seq_lens) with the call's model and the pair lm_ab[g / sweep_B]; everything else is indexed by g.  The slots
+  //     of a sweep differ in their weights only, so its table holds just those, 16 bytes a pair.
+  //   several models (ctcdec_decode_batch_lm_mixed_async): CTA g decodes input row g with lm_slots[lm_slot_of[g]].
+  //     A CTA keeps its own lm_hist_n histories per node, lm_hist_stride ints apart: the slots' largest lm_hist_n
+  //     (0: lm_hist_n).
   int sweep_B;
   const double *lm_ab;              // [P][2]
+  const LmSlot *lm_slots;           // [S]
+  const unsigned char *lm_slot_of;  // [B]
+  int lm_hist_stride;
 };
 
 // control words: 32 ints in L.ctl
@@ -429,7 +452,7 @@ struct Cta {
   uint32_t *s_dmask;    // [KP][WC]: which characters the dictionary lets follow each member
   int WC;
   int space_id;
-  const double *s_ab;      // this CTA's (alpha, beta) in s_ctl: BeamParams::lm_alpha / beta, or its pair of a sweep
+  const double *s_ab;      // this CTA's (alpha, beta) in s_ctl: its LM slot's, or its pair of a sweep
   bool lm_full;
   float lm_cutoff;
   bool lm_char;            // character-based model: no dictionary, an LM term per (member, character)

@@ -46,32 +46,44 @@ namespace ctc {
 // every child shifts in its character's word id; any other child keeps its parent's history.  The terms are those the
 // host hooks give (lm_host.h lm_after_frame / lm_char_row): float(cond_log_prob * alpha) of history + the node's word
 // (word-based, when a space can follow the node) or of history + each label (character-based, the node's row).
-// alpha: the CTA's weight (BeamParams::lm_alpha, or its pair of a sweep).
-CTC_FN float lm_dev_term(const BeamParams &p, double alpha, int *ids, int word) {
-  ids[p.lm_hist_n] = word;
-  return (float)(ngram_cond_ids(p.ngram, ids, p.lm_hist_n + 1) * alpha);
+// m: the CTA's LM slot (its model); alpha: the CTA's weight (the slot's, or its pair of a sweep).  hist: the CTA's
+// histories, m.lm_hist_n ints per node.
+CTC_FN float lm_dev_term(const LmSlot &m, double alpha, int *ids, int word) {
+  ids[m.lm_hist_n] = word;
+  return (float)(ngram_cond_ids(m.ngram, ids, m.lm_hist_n + 1) * alpha);
 }
 
-CTC_FN void lm_dev_root_term(const BeamParams &p, double alpha, float *lm_row, int c) {
+CTC_FN void lm_dev_root_term(const LmSlot *mp, double alpha, float *lm_row, int c) {
+  const LmSlot &m = *mp;
   int ids[kNgramMaxOrder];
-  for (int k = 0; k < p.lm_hist_n; ++k) ids[k] = p.ngram.bos;
-  lm_row[c] = lm_dev_term(p, alpha, ids, p.label_word[c]);
+  for (int k = 0; k < m.lm_hist_n; ++k) ids[k] = m.ngram.bos;
+  lm_row[c] = lm_dev_term(m, alpha, ids, m.label_word[c]);
 }
 
-CTC_FN void lm_dev_node(const BeamParams &p, double alpha, int *hist, float *lm_arena, float *lm_row, int nid, int par,
-                        int ch, int par_state, int arc, int dst) {
-  const int H = p.lm_hist_n;
+CTC_FN void lm_dev_node(const BeamParams &p, const LmSlot *mp, double alpha, int *hist, float *lm_arena, float *lm_row,
+                        int nid, int par, int ch, int par_state, int arc, int dst) {
+  const LmSlot &m = *mp;
+  const int H = m.lm_hist_n;
   int ids[kNgramMaxOrder];
   const int *hp = hist + (size_t)par * H;
   const bool shift = p.lm_char || ch == p.space_id;
   for (int k = 0; k < H; ++k) ids[k] = shift ? (k + 1 < H ? hp[k + 1] : 0) : hp[k];
-  if (shift) ids[H - 1] = p.lm_char ? p.label_word[ch] : p.word_of_state[par_state];
+  if (shift) ids[H - 1] = p.lm_char ? m.label_word[ch] : m.word_of_state[par_state];
   for (int k = 0; k < H; ++k) hist[(size_t)nid * H + k] = ids[k];
   if (p.lm_char) {
-    for (int c = 0; c < p.V; ++c) lm_row[(size_t)nid * p.V + c] = lm_dev_term(p, alpha, ids, p.label_word[c]);
+    for (int c = 0; c < p.V; ++c) lm_row[(size_t)nid * p.V + c] = lm_dev_term(m, alpha, ids, m.label_word[c]);
   } else if (arc & kDictSpace) {
-    lm_arena[nid] = lm_dev_term(p, alpha, ids, p.word_of_state[dst]);
+    lm_arena[nid] = lm_dev_term(m, alpha, ids, m.word_of_state[dst]);
   }
+}
+
+// The LM slot of beam CTA b (BeamParams::lm_slots): its index, and its model -- a slot of the table, or the call's
+// model in the kernel parameters (a __grid_constant__ parameter: its address is taken without a local copy).
+CTC_FN int lm_slot_index(const BeamParams &p, int b) {
+  return p.lm_slot_of ? (int)p.lm_slot_of[b] : p.sweep_B ? b / p.sweep_B : 0;
+}
+CTC_FN const LmSlot *lm_slot(const BeamParams &p, int s) {
+  return p.lm_slots ? p.lm_slots + s : static_cast<const LmSlot *>(&p);
 }
 
 #if defined(CTC_EMULATE) && defined(CTC_STATS)
@@ -427,11 +439,16 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
   c.K = K; c.KP = KP; c.V = V; c.NP = NP; c.W = W; c.blank = p.blank;
   c.WS = WS; c.mch = MERGED;
   c.s_dmask = (uint32_t *)(smem + L.dmask); c.WC = L.WC;
-  c.dict_next = p.dict_next; c.space_id = p.space_id; c.lm_full = false; c.lm_cutoff = kNInf;
-  c.s_ab = (const double *)(smem + H_CTL + C_AB * 4);
-  // sweep of the LM weights: the input row of this CTA, and its (alpha, beta) pair (read once, at the start)
+  // the CTA's LM slot: its model, read where a node or member needs it, and its (alpha, beta) -- the slot's, or its pair
+  // of a sweep -- read once, at the start, into s_ab; in a sweep also the input row of this CTA
   const int bi = LM && p.sweep_B ? b % p.sweep_B : b;
-  const double *const lm_pair = LM && p.lm_ab ? p.lm_ab + 2 * (b / p.sweep_B) : nullptr;
+  const int lm_si = LM ? lm_slot_index(p, b) : 0;
+  const LmSlot *const lm = LM ? lm_slot(p, lm_si) : nullptr;
+  // (inside the frame loop the slot is found again where a node needs it: no pointer stays live across frames)
+  auto cta_slot = [&]() { return lm_slot(p, lm_slot_index(p, b)); };
+  const double *const lm_pair = LM && p.lm_ab ? p.lm_ab + 2 * lm_si : nullptr;
+  c.dict_next = LM ? lm->dict_next : nullptr; c.space_id = p.space_id; c.lm_full = false; c.lm_cutoff = kNInf;
+  c.s_ab = (const double *)(smem + H_CTL + C_AB * 4);
   c.lm_char = LM && p.lm_char != 0; c.lm_row = nullptr;
   int *const s_ctl = c.s_ctl;
 #if !defined(CTC_EMULATE)
@@ -462,7 +479,8 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
   // (a streaming state keeps its histories behind its LM terms, in the same allocation: lm_arena[arena_cap ...])
   int *const lm_hist = !(LM && p.lm_dev) ? nullptr
                        : p.lm_arena_ptrs ? reinterpret_cast<int *>(lm_arena + arena_cap)
-                                         : p.lm_hist + (size_t)b * (size_t)p.arena_stride * (size_t)p.lm_hist_n;
+                                         : p.lm_hist + (size_t)b * (size_t)p.arena_stride *
+                                                           (size_t)(p.lm_hist_stride ? p.lm_hist_stride : p.lm_hist_n);
   int *const s_upd = CTC_SLOT(int, U_NEWINFO);  // staging for the host's answer (free outside R4c..R5: 10 * KP ints)
   // the host's answer: (node, term) pairs -- or, for a character-based model, (node, V terms) entries that are too many
   // for the staging area and are copied from the mapped block straight into the node rows
@@ -557,7 +575,7 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
       ((double *)c.s_logtab)[i] = kLogfTab[i];
     }
     for (int j = tid; j < KP; j += NT) {
-      int node = 0, chr = -1, depth = 0, ts = 0, pslot = -1, anch = -1, dstate = LM ? p.dict_start : 0, jump = -1;
+      int node = 0, chr = -1, depth = 0, ts = 0, pslot = -1, anch = -1, dstate = LM ? lm->dict_start : 0, jump = -1;
       float bprev = kNInf, nbprev = kNInf, score = kNInf, lpc = kNInf;
       if (fresh) {
         if (j == 0) { bprev = 0.0f; score = 0.0f; }  // reference ctc_beam_search_decoder.cpp:43
@@ -571,7 +589,7 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
       c.s_node[j] = node; c.s_chr[j] = chr; c.s_depth[j] = depth; c.s_bprev[j] = bprev; c.s_nbprev[j] = nbprev;
       c.s_score[j] = score; c.s_lpc[j] = lpc; c.s_ts[j] = ts; c.s_pslot[j] = pslot; c.s_anch[j] = anch;
       c.s_dstate[j] = dstate; s_jump[j] = jump;
-      if (LM) for (int w = 0; w < L.WC; ++w) c.s_dmask[j * L.WC + w] = p.dict_mask[(long long)dstate * L.WC + w];
+      if (LM) for (int w = 0; w < L.WC; ++w) c.s_dmask[j * L.WC + w] = lm->dict_mask[(long long)dstate * L.WC + w];
       c.s_lmsp[j] = (LM && !fresh && j < st[0]) ? ld_cg(&lm_arena[node]) : 0.0f;
       c.s_evict[j] = 0;
       s_nodeN[j] = -1;
@@ -600,23 +618,23 @@ CTC_FN void beam_cta_run(const BeamParams &p, const int b, unsigned char *smem) 
       s_ctl[C_FLAGS] = fresh ? 0 : st[3];
       if (LM) {
         double *const ab = (double *)(s_ctl + C_AB);
-        ab[0] = lm_pair ? lm_pair[0] : p.lm_alpha;
-        ab[1] = lm_pair ? lm_pair[1] : p.beta;
+        ab[0] = lm_pair ? lm_pair[0] : lm->lm_alpha;
+        ab[1] = lm_pair ? lm_pair[1] : lm->beta;
       }
       s_ctl[C_KMIN] = (int)0xFFFFFFFFu;
       s_ctl[C_SMIN] = (int)0xFFFFFFFFu;
       if (fresh) {  // root node (reference path_trie.cpp:11-30)
         Node root; root.parent = -1; root.chr = -1; root.lpc = kNInf; root.ts = 0; root.jump = -1;
         store_node(&nodes[0], root);
-        if (LM) { dstate_arena[0] = p.dict_start; lm_arena[0] = 0.0f; }
+        if (LM) { dstate_arena[0] = lm->dict_start; lm_arena[0] = 0.0f; }
       }
     }
     // device n-gram scorer, before the first frame of an utterance or stream: the root's history (the "<s>" padding
     // of Scorer::make_ngram) and, for a character-based model, its row of LM terms
     if (LM && p.lm_dev && abs_t0 == 0) {
-      for (int k = tid; k < p.lm_hist_n; k += NT) lm_hist[k] = p.ngram.bos;
+      for (int k = tid; k < lm->lm_hist_n; k += NT) lm_hist[k] = lm->ngram.bos;
       if (p.lm_char)
-        for (int x = tid; x < V; x += NT) lm_dev_root_term(p, lm_pair ? lm_pair[0] : p.lm_alpha, lm_row, x);
+        for (int x = tid; x < V; x += NT) lm_dev_root_term(lm, lm_pair ? lm_pair[0] : lm->lm_alpha, lm_row, x);
     }
   }
 #if !defined(CTC_EMULATE)

@@ -31,8 +31,9 @@ namespace ctc {
 // two co-resident CTAs per SM (one for NT = 1024, three for NT = 128): 128 registers per thread up to NT = 256, 64 at NT = 512.
 // A config-2 batch of 256 utterances is 1.73 CTAs per SM, and the frame loop wants its registers.
 // KPT: beam size rounded up to 32 as a compile-time constant (0 = generic), TIMING: per-region cycle counters.
+// (__grid_constant__: a scorer CTA without a slot table reads the call's model through a pointer to the parameters)
 template <int NT, bool SORTED, bool LM, int KPT, bool TIMING>
-__global__ void __launch_bounds__(NT, (NT >= 1024 ? 1 : NT <= 128 ? 3 : 2)) beam_kernel(const BeamParams p) {
+__global__ void __launch_bounds__(NT, (NT >= 1024 ? 1 : NT <= 128 ? 3 : 2)) beam_kernel(const __grid_constant__ BeamParams p) {
   extern __shared__ __align__(128) unsigned char smem[];
   beam_cta_run<NT, SORTED, LM, KPT, TIMING>(p, (int)blockIdx.x, smem);
 }
@@ -114,6 +115,32 @@ __global__ void sweep_pairs_kernel(const SweepPairArgs a) {
   a.tab[2 * (a.p0 + i) + 1] = a.ab[2 * i + 1];
 }
 
+// The LM slots of a decode over several models (ctcdec_decode_batch_lm_mixed_async) and each utterance's slot index
+// into the workspace, from the launch parameters: the call copies nothing from host memory, and a graph replays the
+// models and weights it captured.  All slots travel in one launch (kMaxLmSlots of them: CTCDEC_LM_MIXED_MAX_MODELS),
+// the indices kSlotIndexPerLaunch per launch.
+constexpr int kMaxLmSlots = CTCDEC_LM_MIXED_MAX_MODELS;
+constexpr size_t kLmSlotBytes = 256;  // workspace bytes per slot (ctcdec_lm_mixed_workspace_bytes)
+static_assert(sizeof(LmSlot) <= kLmSlotBytes, "an LM slot outgrew its workspace share");
+struct LmSlotArgs {
+  LmSlot *tab;
+  int S;
+  LmSlot slot[kMaxLmSlots];
+};
+static_assert(sizeof(LmSlotArgs) <= 4096, "the slots must fit the kernel parameters");
+__global__ void lm_slots_kernel(const LmSlotArgs a) {
+  if ((int)threadIdx.x < a.S) a.tab[threadIdx.x] = a.slot[threadIdx.x];
+}
+constexpr int kSlotIndexPerLaunch = 4000;
+struct SlotIndexArgs {
+  unsigned char *tab;
+  int b0, n;
+  unsigned char index[kSlotIndexPerLaunch];
+};
+__global__ void lm_slot_index_kernel(const SlotIndexArgs a) {
+  for (int i = (int)threadIdx.x; i < a.n; i += (int)blockDim.x) a.tab[a.b0 + i] = a.index[i];
+}
+
 // Sweep: the prune scan's flags of the B input rows (slice 0 of flags [P][B]) into the other P - 1 slices, before the
 // beam and finalize kernels OR in each CTA's own bits.
 __global__ void sweep_flags_kernel(int32_t *flags, int B, long long n) {
@@ -123,13 +150,16 @@ __global__ void sweep_flags_kernel(int32_t *flags, int B, long long n) {
 
 // Read-out of an ARPA scorer's results (ngram_readout_row, reference DecoderState::decode): one thread per [B, K] result
 // row, rows p >= n_results[b] skipped, scores rescored in place.  Each row is a serial chain of hash probes (about
-// words x order of them).  SWEEP: row r takes the pair ab[r / (pair_B x K)] instead of alpha / beta.  (A compile-time
-// choice: the two doubles loaded per row stay live across the row's walks and cost the kernel a spill, which the
-// single-pair instantiation is kept free of.)
+// words x order of them).  Rows take their utterance's LM slot in the per-row instantiations (compile-time choices:
+// what a row loads stays live across its walks, and the single-model instantiation is kept free of that):
+//   kReadSweep: row r takes the pair ab[r / (pair_B x K)] instead of alpha / beta (the model is m, f);
+//   kReadSlots: row r of utterance b takes model, front end and weights of slots[slot_of[b]].
 constexpr int kReadoutThreads = 128;
-template <bool SWEEP>
+enum { kReadOne = 0, kReadSweep = 1, kReadSlots = 2 };
+template <int MODE>
 __global__ void __launch_bounds__(kReadoutThreads) lm_readout_kernel(const NgramView m, const NgramFront f, double alpha,
                                                                      double beta, const double *ab, int pair_B,
+                                                                     const LmSlot *slots, const unsigned char *slot_of,
                                                                      const int32_t *tokens,
                                                                      const int32_t *lens, const int32_t *n_results,
                                                                      float *scores, int B, int K, int row_stride) {
@@ -137,7 +167,12 @@ __global__ void __launch_bounds__(kReadoutThreads) lm_readout_kernel(const Ngram
   if (r >= (long long)B * K) return;
   const int b = (int)(r / K), p = (int)(r % K);
   if (p >= n_results[b]) return;
-  if (SWEEP) {
+  if (MODE == kReadSlots) {
+    const LmSlot &sl = slots[slot_of[b]];
+    scores[r] = ngram_readout_row(sl.ngram, sl.front, tokens + r * row_stride, lens[r], scores[r], sl.lm_alpha, sl.beta);
+    return;
+  }
+  if (MODE == kReadSweep) {
     const int q = b / pair_B;
     alpha = ab[2 * q];
     beta = ab[2 * q + 1];
@@ -674,18 +709,26 @@ static int ensure_ngram_on_device(HostScorer *sc, int device) {
 // Enqueues the read-out of an ARPA scorer's [B, K] result rows (row_stride columns each) on s; the scorer's tables must
 // be on the current device.  alpha and beta are the scorer's values now, or, for a sweep, the device table ab [P][2]
 // with pair_B utterances per pair.
+// For a decode over several models, slots / slot_of are the device tables of the LM slots and of each utterance's slot
+// (sc is then unused).
 static int launch_readout(const HostScorer *sc, const int32_t *tokens, const int32_t *lens, const int32_t *n_results,
                           float *scores, int B, int K, int row_stride, cudaStream_t s, const double *ab = nullptr,
-                          int pair_B = 0) {
+                          int pair_B = 0, const LmSlot *slots = nullptr, const unsigned char *slot_of = nullptr) {
   const long long rows = (long long)B * K;
   if (rows == 0) return CTCDEC_OK;
   const unsigned grid = (unsigned)((rows + kReadoutThreads - 1) / kReadoutThreads);
-  if (ab)
-    lm_readout_kernel<true><<<grid, kReadoutThreads, 0, s>>>(sc->d_view, sc->d_front, 0.0, 0.0, ab, pair_B, tokens,
-                                                             lens, n_results, scores, B, K, row_stride);
+  if (slots)
+    lm_readout_kernel<kReadSlots><<<grid, kReadoutThreads, 0, s>>>(NgramView(), NgramFront(), 0.0, 0.0, nullptr, 1,
+                                                                   slots, slot_of, tokens, lens, n_results, scores, B,
+                                                                   K, row_stride);
+  else if (ab)
+    lm_readout_kernel<kReadSweep><<<grid, kReadoutThreads, 0, s>>>(sc->d_view, sc->d_front, 0.0, 0.0, ab, pair_B,
+                                                                   nullptr, nullptr, tokens, lens, n_results, scores,
+                                                                   B, K, row_stride);
   else
-    lm_readout_kernel<false><<<grid, kReadoutThreads, 0, s>>>(sc->d_view, sc->d_front, sc->alpha, sc->beta, nullptr,
-                                                              1, tokens, lens, n_results, scores, B, K, row_stride);
+    lm_readout_kernel<kReadOne><<<grid, kReadoutThreads, 0, s>>>(sc->d_view, sc->d_front, sc->alpha, sc->beta, nullptr,
+                                                                 1, nullptr, nullptr, tokens, lens, n_results, scores,
+                                                                 B, K, row_stride);
   CU(cudaGetLastError());
   return CTCDEC_OK;
 }
@@ -781,15 +824,45 @@ static void flat_arenas(BeamParams &bp, const Plan &pl, unsigned char *ws) {
   bp.arena_cap = (int)pl.arena_stride;
 }
 
+// The scorer's model and weights as an LM slot (beam_core.cuh): its dictionary must be on the device, and for an n-gram
+// scorer its tables too.
+static LmSlot scorer_slot(const HostScorer &sc) {
+  LmSlot m;
+  m.dict_next = sc.d_next; m.dict_mask = sc.d_mask; m.dict_start = sc.dict.start; m.beta = sc.beta;
+  m.lm_alpha = 0.0; m.word_of_state = nullptr; m.label_word = nullptr; m.lm_hist_n = 0;
+  if (sc.ngram) {
+    m.lm_alpha = sc.alpha; m.ngram = sc.d_view; m.front = sc.d_front;
+    m.word_of_state = sc.d_word_of_state; m.label_word = sc.d_label_word; m.lm_hist_n = sc.max_order - 1;
+  }
+  return m;
+}
+
+// The LM slots of S scorers (each with its alpha and beta as they are now) into the device table slots, and the slot
+// index of each of B utterances or streams into slot_of, enqueued on s from kernel launch parameters.
+static int upload_slots(HostScorer *const *scs, int S, const unsigned char *index, int B, LmSlot *slots,
+                        unsigned char *slot_of, cudaStream_t s) {
+  LmSlotArgs a;
+  memset(&a, 0, sizeof(a));
+  a.tab = slots; a.S = S;
+  for (int i = 0; i < S; ++i) a.slot[i] = scorer_slot(*scs[i]);
+  lm_slots_kernel<<<1, kMaxLmSlots, 0, s>>>(a);
+  CU(cudaGetLastError());
+  for (int b0 = 0; b0 < B; b0 += kSlotIndexPerLaunch) {
+    SlotIndexArgs x;
+    x.tab = slot_of; x.b0 = b0; x.n = std::min(kSlotIndexPerLaunch, B - b0);
+    memcpy(x.index, index + b0, (size_t)x.n);
+    lm_slot_index_kernel<<<1, 256, 0, s>>>(x);
+    CU(cudaGetLastError());
+  }
+  return CTCDEC_OK;
+}
+
 // The scorer's part of the kernel parameters (its dictionary must be on the device): the dictionary and the word
 // bonus, and for an n-gram scorer, whose tables must be on the device too, the model the beam kernel scores with.
 static void attach_scorer(BeamParams &bp, const HostScorer &sc) {
-  bp.dict_next = sc.d_next; bp.dict_mask = sc.d_mask; bp.dict_wc = sc.dict.wc; bp.dict_start = sc.dict.start;
-  bp.space_id = sc.space_id; bp.beta = sc.beta; bp.lm_char = sc.is_character_based ? 1 : 0;
-  if (sc.ngram) {
-    bp.lm_dev = 1; bp.lm_alpha = sc.alpha; bp.ngram = sc.d_view;
-    bp.word_of_state = sc.d_word_of_state; bp.label_word = sc.d_label_word; bp.lm_hist_n = sc.max_order - 1;
-  }
+  static_cast<LmSlot &>(bp) = scorer_slot(sc);
+  bp.dict_wc = sc.dict.wc; bp.space_id = sc.space_id; bp.lm_char = sc.is_character_based ? 1 : 0;
+  bp.lm_dev = sc.ngram ? 1 : 0;
 }
 
 // The pinned exchange blocks of a hook scorer's handshake (beam_core.cuh) for B utterances, in the cache c, and the
@@ -1211,20 +1284,69 @@ int ctcdec_state_frames(const void *state, int *frames) {
   return CTCDEC_OK;
 }
 
-// all states of one call: non-NULL, distinct, same configuration, scorer and device
+// Two scorers of one call that are not the same object: both n-gram scorers from ctcdec_scorer_create_arpa, of one kind
+// and built for the same labels (each utterance or stream then decodes with its own through its LM slot).  i: the
+// index named in the message.
+static int check_scorer_pair(const HostScorer *a, const HostScorer *b, const char *what, int i) {
+  if (!a->ngram || !b->ngram)
+    return fail(CTCDEC_E_UNSUPPORTED, "a hook scorer cannot share a call with another scorer: its terms come from the "
+                "host's per-frame handshake");
+  if (a->is_character_based != b->is_character_based)
+    return fail(CTCDEC_E_UNSUPPORTED, "%s %d and 0 of one call are not both word-based or both character-based", what,
+                i);
+  if (a->labels != b->labels) return fail(CTCDEC_E_INVALID, "%s %d and 0 were built for different labels", what, i);
+  return CTCDEC_OK;
+}
+
+// The distinct scorers of a call's states (scs, at most kMaxLmSlots of them) and the index of each stream's among them.
+static void stream_scorers(void *const *states, int B, std::vector<HostScorer *> *scs,
+                           std::vector<unsigned char> *slot_of) {
+  scs->clear();
+  slot_of->assign((size_t)B, 0);
+  for (int b = 0; b < B; ++b) {
+    HostScorer *sc = static_cast<const StreamState *>(states[b])->sc;
+    size_t i = 0;
+    while (i < scs->size() && (*scs)[i] != sc) ++i;
+    if (i == scs->size()) scs->push_back(sc);
+    (*slot_of)[b] = (unsigned char)i;
+  }
+}
+
+// all states of one call: non-NULL, distinct, same configuration and device; their scorers one object (or none), or
+// n-gram scorers that check_scorer_pair lets share a call, at most kMaxLmSlots different ones
 static int check_states(void *const *states, int B) {
   if (!states) return fail(CTCDEC_E_INVALID, "states is NULL");
   for (int b = 0; b < B; ++b)
     if (!states[b]) return fail(CTCDEC_E_INVALID, "states[%d] is NULL", b);
   const StreamState *s0 = static_cast<const StreamState *>(states[0]);
+  std::vector<const HostScorer *> seen(1, s0->sc);
   for (int b = 1; b < B; ++b) {
     const StreamState *sb = static_cast<const StreamState *>(states[b]);
-    if (memcmp(&sb->cfg, &s0->cfg, sizeof(s0->cfg)) != 0 || sb->device != s0->device || sb->sc != s0->sc)
-      return fail(CTCDEC_E_UNSUPPORTED, "all states of one call must come from the same decoder configuration, scorer and device");
+    if (memcmp(&sb->cfg, &s0->cfg, sizeof(s0->cfg)) != 0 || sb->device != s0->device)
+      return fail(CTCDEC_E_UNSUPPORTED, "all states of one call must come from the same decoder configuration and device");
+    if (sb->sc != s0->sc) {
+      if (!sb->sc || !s0->sc)
+        return fail(CTCDEC_E_UNSUPPORTED, "states with a scorer and states without one cannot share a call");
+      int rc = check_scorer_pair(s0->sc, sb->sc, "the scorers of states", b);
+      if (rc) return rc;
+      if (std::find(seen.begin(), seen.end(), sb->sc) == seen.end()) seen.push_back(sb->sc);
+      if ((int)seen.size() > kMaxLmSlots)
+        return fail(CTCDEC_E_UNSUPPORTED, "the states of one call use more than %d different scorers "
+                    "(CTCDEC_LM_MIXED_MAX_MODELS)", kMaxLmSlots);
+    }
     for (int a = 0; a < b; ++a)
       if (states[a] == states[b]) return fail(CTCDEC_E_INVALID, "states[%d] and states[%d] are the same object", a, b);
   }
   return CTCDEC_OK;
+}
+
+// Device bytes of the LM slots of a streaming call whose states use several scorers (0 for one scorer or none): the
+// streams' slot indices, then one slot per scorer, each region 256-byte aligned.
+static size_t stream_slot_bytes(void *const *states, int B) {
+  std::vector<HostScorer *> scs;
+  std::vector<unsigned char> slot_of;
+  stream_scorers(states, B, &scs, &slot_of);
+  return scs.size() > 1 ? al256((size_t)B) + al256(scs.size() * kLmSlotBytes) : 0;
 }
 
 // order work on stream s after the pending device-path calls of these states
@@ -1299,6 +1421,8 @@ struct ChunkBuffers {
   int kind;
   unsigned char *ws;  // the plan's pruned rows and characters (a workspace laid out by the plan, up to off_arena)
   unsigned char *tab; // stream_tab_layout(B).total bytes
+  unsigned char *slot_tab;  // states of several scorers: stream_slot_bytes bytes for their slot indices and LM slots,
+                            // else NULL
   DecodeOut out;
   int out_T;
 };
@@ -1323,7 +1447,13 @@ static int stream_chunk_step(const ctcdec_config &cfg, Plan &pl, void *const *st
   }
   if ((rc = grow_arenas(states, B, clen.data(), s))) return rc;
   HostScorer *const sc = static_cast<StreamState *>(states[0])->sc;
-  if (sc && (rc = ensure_dict_on_device(sc, static_cast<StreamState *>(states[0])->device))) return rc;
+  const int device = static_cast<StreamState *>(states[0])->device;
+  std::vector<HostScorer *> scs;
+  std::vector<unsigned char> slot_of;
+  stream_scorers(states, B, &scs, &slot_of);
+  for (HostScorer *si : scs)
+    if (si && ((rc = ensure_dict_on_device(si, device)) || (si->ngram && (rc = ensure_ngram_on_device(si, device)))))
+      return rc;
   const StreamTabLayout L = stream_tab_layout(B);
   for (int b0 = 0; b0 < B; b0 += kTabPerLaunch) {
     StreamTabArgs a;
@@ -1350,11 +1480,18 @@ static int stream_chunk_step(const ctcdec_config &cfg, Plan &pl, void *const *st
   bp.finalize = io.tab + L.fin;
   bp.fresh = 0;
   if (sc && T > 0) {
-    if (sc->ngram && (rc = ensure_ngram_on_device(sc, static_cast<StreamState *>(states[0])->device))) return rc;
     attach_scorer(bp, *sc);
     bp.lm_arena_ptrs = (float *const *)(io.tab + L.lmar);
     bp.dstate_ptrs = (int *const *)(io.tab + L.dst);
     if (sc->is_character_based) bp.lm_row_ptrs = (float *const *)(io.tab + L.rows);
+  }
+  if (scs.size() > 1) {
+    // streams of several scorers: stream b decodes with the LM slot of its own scorer, its weights as they are now
+    // (each stream keeps its own order - 1 histories behind its LM terms)
+    unsigned char *const d_slot_of = io.slot_tab;
+    LmSlot *const slots = reinterpret_cast<LmSlot *>(io.slot_tab + al256((size_t)B));
+    if ((rc = upload_slots(scs.data(), (int)scs.size(), slot_of.data(), B, slots, d_slot_of, s))) return rc;
+    bp.lm_slots = slots; bp.lm_slot_of = d_slot_of;
   }
   if (sc && !sc->ngram && T > 0) {
     // hook scorer: one persistent launch per chunk, hand shake after EVERY frame (the frame after the chunk's last
@@ -1404,7 +1541,8 @@ int ctcdec_decode_stream_host(const float *probs, const int32_t *seq_lens, int B
   if ((rc = ensure(c, kBufTimesteps, n_out * 4 + 256))) return rc;
   if ((rc = ensure(c, kBufSmall, small_bytes(B, K)))) return rc;
   if ((rc = ensure(c, kBufWork, pl.off_arena + 512))) return rc;  // only the lp / idx part of the plan is used
-  if ((rc = ensure(c, kBufStreamTab, stream_tab_layout(B).total + 256))) return rc;
+  const size_t slot_bytes = stream_slot_bytes(states, B);
+  if ((rc = ensure(c, kBufStreamTab, stream_tab_layout(B).total + slot_bytes + 256))) return rc;
   float *d_probs = (float *)c.buf[kBufInput];
   int *d_tok = (int *)c.buf[kBufTokens], *d_ts = (int *)c.buf[kBufTimesteps];
   const SmallOut d = small_out(c.buf[kBufSmall], B, K);
@@ -1413,6 +1551,7 @@ int ctcdec_decode_stream_host(const float *probs, const int32_t *seq_lens, int B
   io.chunk = d_probs; io.kind = IN_F32;
   io.ws = align256(c.buf[kBufWork]);
   io.tab = (unsigned char *)c.buf[kBufStreamTab];
+  io.slot_tab = slot_bytes ? io.tab + stream_tab_layout(B).total : nullptr;
   io.out = DecodeOut{d_tok, d_ts, d.scores, d.lens, d.n_results, d.flags};
   io.out_T = out_T;
   if ((rc = stream_chunk_step(cfg, pl, states, B, T, seq_lens, is_eos, io, &c, s))) return rc;
@@ -1435,10 +1574,16 @@ int ctcdec_decode_stream_host(const float *probs, const int32_t *seq_lens, int B
       }
     }
     CU(cudaStreamSynchronize(s));
-    if (sc) {  // reported scores of the finished streams: approx_ctc (reference ctc_beam_search_decoder.cpp:173-208)
+    if (sc) {  // reported scores of the finished streams: approx_ctc (reference ctc_beam_search_decoder.cpp:173-208),
+               // each with its own scorer
+      std::vector<HostScorer *> scs;
+      std::vector<unsigned char> slot_of;
+      stream_scorers(states, B, &scs, &slot_of);
       std::vector<int> nres_eos(B);
-      for (int b = 0; b < B; ++b) nres_eos[b] = is_eos[b] ? h.n_results[b] : 0;
-      lm_rescore_batch(*sc, B, K, out_T, nres_eos.data(), tokens, lens, scores);
+      for (size_t i = 0; i < scs.size(); ++i) {
+        for (int b = 0; b < B; ++b) nres_eos[b] = is_eos[b] && slot_of[b] == i ? h.n_results[b] : 0;
+        lm_rescore_batch(*scs[i], B, K, out_T, nres_eos.data(), tokens, lens, scores);
+      }
     }
     if (n_results) memcpy(n_results, h.n_results, (size_t)B * 4);
     if (flags) memcpy(flags, h.flags, (size_t)B * 4);
@@ -1450,8 +1595,11 @@ int ctcdec_decode_stream_host(const float *probs, const int32_t *seq_lens, int B
   return CTCDEC_OK;
 }
 
-// device scratch of ctcdec_decode_stream_device: the plan's pruned rows / characters, then the per-call tables
-static size_t stream_workspace_bytes(const Plan &pl, int B) { return al256(pl.off_arena) + stream_tab_layout(B).total + 256; }
+// device scratch of ctcdec_decode_stream_device: the plan's pruned rows / characters, then the per-call tables, then
+// for states of several scorers their LM slots (slot_bytes, stream_slot_bytes)
+static size_t stream_workspace_bytes(const Plan &pl, int B, size_t slot_bytes = 0) {
+  return al256(pl.off_arena) + stream_tab_layout(B).total + slot_bytes + 256;
+}
 
 int ctcdec_stream_workspace_bytes(const ctcdec_config *cfg, int B, int T, size_t *bytes) {
   Plan pl;
@@ -1459,6 +1607,18 @@ int ctcdec_stream_workspace_bytes(const ctcdec_config *cfg, int B, int T, size_t
   if (rc) return rc;
   if (!bytes) return fail(CTCDEC_E_INVALID, "bytes is NULL");
   *bytes = stream_workspace_bytes(pl, B);
+  return CTCDEC_OK;
+}
+
+int ctcdec_stream_states_workspace_bytes(void *const *states, int B, int T, size_t *bytes) {
+  if (B <= 0) return fail(CTCDEC_E_INVALID, "batch %d: the states decide the workspace, at least one is needed", B);
+  int rc = check_states(states, B);
+  if (rc) return rc;
+  const StreamState *s0 = static_cast<const StreamState *>(states[0]);
+  Plan pl;
+  if ((rc = make_plan(&s0->cfg, B, T, &pl))) return rc;
+  if (!bytes) return fail(CTCDEC_E_INVALID, "bytes is NULL");
+  *bytes = stream_workspace_bytes(pl, B, stream_slot_bytes(states, B));
   return CTCDEC_OK;
 }
 
@@ -1501,7 +1661,8 @@ int ctcdec_decode_stream_device(const void *probs, int dtype, const int32_t *seq
   if (any_eos && (!tokens || !timesteps || !scores || !lens)) return fail(CTCDEC_E_INVALID, "an output pointer is NULL");
   if ((rc = check_current_device(s0))) return rc;
   unsigned char *ws = nullptr;
-  if ((rc = workspace_start(workspace, workspace_bytes, stream_workspace_bytes(pl, B), &ws))) return rc;
+  const size_t slot_bytes = stream_slot_bytes(states, B);
+  if ((rc = workspace_start(workspace, workspace_bytes, stream_workspace_bytes(pl, B, slot_bytes), &ws))) return rc;
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
   std::lock_guard<std::mutex> lock(g_mu[s0->device]);
   if ((rc = wait_device_work(states, B, s))) return rc;
@@ -1509,12 +1670,20 @@ int ctcdec_decode_stream_device(const void *probs, int dtype, const int32_t *seq
   io.chunk = probs; io.kind = kind;
   io.ws = ws;
   io.tab = ws + al256(pl.off_arena);
+  io.slot_tab = slot_bytes ? io.tab + stream_tab_layout(B).total : nullptr;
   io.out = DecodeOut{tokens, timesteps, scores, lens, n_results, flags};
   io.out_T = out_T;
   if ((rc = stream_chunk_step(cfg, pl, states, B, T, seq_lens, is_eos, io, nullptr, s))) return rc;
   if (sc && any_eos) {  // the eos streams' reported scores (the other streams' n_results are 0: their rows are skipped)
     if ((rc = ensure_ngram_on_device(sc, s0->device))) return rc;
-    if ((rc = launch_readout(sc, tokens, lens, n_results, scores, B, cfg.beam_size, out_T, s))) return rc;
+    if (slot_bytes) {  // each stream's rows with its own scorer's slot (written by the chunk step, also with T = 0)
+      const LmSlot *slots = reinterpret_cast<const LmSlot *>(io.slot_tab + al256((size_t)B));
+      rc = launch_readout(nullptr, tokens, lens, n_results, scores, B, cfg.beam_size, out_T, s, nullptr, 0, slots,
+                          io.slot_tab);
+    } else {
+      rc = launch_readout(sc, tokens, lens, n_results, scores, B, cfg.beam_size, out_T, s);
+    }
+    if (rc) return rc;
   }
   return record_device_work(states, B, s);
 }
@@ -1686,6 +1855,11 @@ struct LmBuffers {
   // and the outputs above then hold P x B utterances (pair-major), the input rows B
   int P = 1;
   const double *lm_ab = nullptr;
+  // several models (ctcdec_decode_batch_lm_mixed_async): the device tables of the LM slots and of each utterance's
+  // slot; lm_hist holds the slots' largest order - 1 ids per node
+  const LmSlot *lm_slots = nullptr;
+  const unsigned char *lm_slot_of = nullptr;
+  int lm_hist_stride = 0;
 };
 
 // One offline scorer decode from the point where the input is on the device, enqueued on s; shared by both scorer
@@ -1719,6 +1893,7 @@ static int lm_batch_step(const ctcdec_config *cfg, const Plan &pl, HostScorer *s
     // blocks, host workers or handshake
     bp.lm_hist = io.lm_hist;
     bp.sweep_B = io.lm_ab ? B : 0; bp.lm_ab = io.lm_ab;
+    bp.lm_slots = io.lm_slots; bp.lm_slot_of = io.lm_slot_of; bp.lm_hist_stride = io.lm_hist_stride;
     if ((rc = launch_beam(bp, pl, G, s))) return rc;
     return launch_finalize(bp, G, s);
   }
@@ -1998,24 +2173,97 @@ int ctcdec_decode_batch_lm_device(const ctcdec_config *cfg, void *scorer, const 
   return check_error_flags(h.flags, B);
 }
 
-// ctcdec_decode_batch_lm_device_async (P = 0: the scorer's alpha and beta) and ctcdec_decode_batch_lm_sweep_async (P >= 1
-// host pairs: outputs [P, B, ...]).
+// the utterances' slot indices (checked to lie in [0, S)) as bytes
+static std::vector<unsigned char> lm_index_bytes(const int32_t *lm_index, int B) {
+  std::vector<unsigned char> v((size_t)B);
+  for (int b = 0; b < B; ++b) v[b] = (unsigned char)lm_index[b];
+  return v;
+}
+
+// A decode over several models (ctcdec_decode_batch_lm_mixed_async): the host arrays of the call.
+struct MixedCall {
+  void *const *scorers;
+  int S;
+  const int32_t *lm_index;
+};
+
+// The checks of a decode over several models and its workspace: the plan of a B-utterance decode with a scorer, the
+// workspace of the scorer with the largest order (*rep: its per-node histories have the stride every slot fits in),
+// then the S slots and the B slot indices at w->total (*bytes: the whole workspace the caller provides).  *single: all
+// scorers are one object, which decodes as ctcdec_decode_batch_lm_device_async does, in its workspace.
+static int lm_mixed_plan(const ctcdec_config *cfg, void *const *scorers, int S, int B, int T, Plan *pl, LmWorkspace *w,
+                         size_t *bytes, HostScorer **rep, bool *single) {
+  if (!scorers) return fail(CTCDEC_E_INVALID, "scorers is NULL");
+  if (S < 1 || S > kMaxLmSlots)
+    return fail(CTCDEC_E_INVALID, "%d scorers: a call takes 1 to %d (CTCDEC_LM_MIXED_MAX_MODELS)", S, kMaxLmSlots);
+  for (int i = 0; i < S; ++i)
+    if (!scorers[i]) return fail(CTCDEC_E_INVALID, "scorers[%d] is NULL", i);
+  const HostScorer *s0 = static_cast<const HostScorer *>(scorers[0]);
+  *rep = static_cast<HostScorer *>(scorers[0]);
+  *single = true;
+  for (int i = 1; i < S; ++i) {
+    HostScorer *si = static_cast<HostScorer *>(scorers[i]);
+    if (si == s0) continue;
+    *single = false;
+    const int rc = check_scorer_pair(s0, si, "scorers", i);
+    if (rc) return rc;
+    if (si->max_order > (*rep)->max_order) *rep = si;
+  }
+  int rc = lm_device_plan(cfg, *rep, B, T, pl, w);
+  if (rc) return rc;
+  *bytes = *single ? w->total + 256 : w->total + al256((size_t)S * kLmSlotBytes) + al256((size_t)B) + 256;
+  return CTCDEC_OK;
+}
+
+int ctcdec_lm_mixed_workspace_bytes(const ctcdec_config *cfg, void *const *scorers, int S, int B, int T,
+                                    size_t *bytes) {
+  Plan pl;
+  LmWorkspace w;
+  size_t need = 0;
+  HostScorer *rep = nullptr;
+  bool single = false;
+  const int rc = lm_mixed_plan(cfg, scorers, S, B, T, &pl, &w, &need, &rep, &single);
+  if (rc) return rc;
+  if (!bytes) return fail(CTCDEC_E_INVALID, "bytes is NULL");
+  *bytes = need;
+  return CTCDEC_OK;
+}
+
+// ctcdec_decode_batch_lm_device_async (P = 0: the scorer's alpha and beta), ctcdec_decode_batch_lm_sweep_async (P >= 1
+// host pairs: outputs [P, B, ...]) and ctcdec_decode_batch_lm_mixed_async (mx: utterance b with
+// mx->scorers[mx->lm_index[b]]; scorer NULL).
 static int lm_decode_async(const ctcdec_config *cfg, void *scorer, const void *input, int dtype,
                            const int32_t *seq_lens, int B, int T, const double *alphas, const double *betas, int P,
                            int32_t *tokens, int32_t *timesteps, float *scores, int32_t *lens, int32_t *n_results,
-                           int32_t *flags, float *log_probs_out, void *workspace, size_t workspace_bytes, void *stream) {
-  if (!scorer) return fail(CTCDEC_E_INVALID, "scorer is NULL");
-  int kind = 0;
-  int rc = input_kind(dtype, true, &kind);
-  if (rc) return rc;
-  const bool sweep = P > 0;
+                           int32_t *flags, float *log_probs_out, void *workspace, size_t workspace_bytes, void *stream,
+                           const MixedCall *mx = nullptr) {
+  HostScorer *rep = nullptr;
+  bool single = true;
   Plan pl;
   LmWorkspace w;
   size_t need_bytes = 0;
-  rc = sweep ? lm_sweep_plan(cfg, scorer, B, T, P, &pl, &w, &need_bytes) : lm_device_plan(cfg, scorer, B, T, &pl, &w);
-  if (rc) return rc;
-  if (!sweep) need_bytes = w.total + 256;
-  HostScorer *sc = static_cast<HostScorer *>(scorer);
+  int rc = CTCDEC_OK;
+  if (mx) {
+    if ((rc = lm_mixed_plan(cfg, mx->scorers, mx->S, B, T, &pl, &w, &need_bytes, &rep, &single))) return rc;
+    if (B > 0 && !mx->lm_index) return fail(CTCDEC_E_INVALID, "lm_index (host int32[B]) is NULL");
+    for (int b = 0; b < B; ++b)
+      if (mx->lm_index[b] < 0 || mx->lm_index[b] >= mx->S)
+        return fail(CTCDEC_E_INVALID, "lm_index[%d] = %d outside [0, %d)", b, mx->lm_index[b], mx->S);
+    if (single) {
+      scorer = mx->scorers[0];
+      mx = nullptr;
+    }
+  }
+  if (!scorer && !mx) return fail(CTCDEC_E_INVALID, "scorer is NULL");
+  int kind = 0;
+  if ((rc = input_kind(dtype, true, &kind))) return rc;
+  const bool sweep = P > 0;
+  if (!mx) {
+    rc = sweep ? lm_sweep_plan(cfg, scorer, B, T, P, &pl, &w, &need_bytes) : lm_device_plan(cfg, scorer, B, T, &pl, &w);
+    if (rc) return rc;
+    if (!sweep) need_bytes = w.total + 256;
+  }
+  HostScorer *sc = mx ? rep : static_cast<HostScorer *>(scorer);
   if (!sc->ngram)
     return fail(CTCDEC_E_UNSUPPORTED, "the asynchronous scorer decode takes a scorer from ctcdec_scorer_create_arpa only: "
                 "a hook scorer needs the host during the call (use ctcdec_decode_batch_lm_device)");
@@ -2032,9 +2280,14 @@ static int lm_decode_async(const ctcdec_config *cfg, void *scorer, const void *i
   std::lock_guard<std::mutex> lock(g_mu[device]);
   // nothing that allocates, uploads or synchronises may run while the stream is captured: the scorer's tables must be
   // on this device already (the first decode puts them there)
-  if (capturing != cudaStreamCaptureStatusNone &&
-      !(sc->d_next && sc->device == device && sc->d_ngram && sc->ngram_device == device))
-    return fail(CTCDEC_E_UNSUPPORTED, "the scorer's tables are not on device %d yet: %s", device, kCaptureFirst);
+  const int n_sc = mx ? mx->S : 1;
+  for (int i = 0; i < n_sc; ++i) {
+    HostScorer *si = mx ? static_cast<HostScorer *>(mx->scorers[i]) : sc;
+    if (capturing != cudaStreamCaptureStatusNone &&
+        !(si->d_next && si->device == device && si->d_ngram && si->ngram_device == device))
+      return fail(CTCDEC_E_UNSUPPORTED, "the scorer's tables are not on device %d yet: %s", device, kCaptureFirst);
+    if (mx && ((rc = ensure_dict_on_device(si, device)) || (rc = ensure_ngram_on_device(si, device)))) return rc;
+  }
   struct CaptureGuard {
     explicit CaptureGuard(bool on) { g_capturing = on; }
     ~CaptureGuard() { g_capturing = false; }
@@ -2055,9 +2308,20 @@ static int lm_decode_async(const ctcdec_config *cfg, void *scorer, const void *i
     }
     io.P = P; io.lm_ab = tab;
   }
+  if (mx) {
+    // the slots: each scorer's model with its alpha and beta as they are now
+    LmSlot *const slots = reinterpret_cast<LmSlot *>(io.ws + w.total);
+    unsigned char *const slot_of = io.ws + w.total + al256((size_t)mx->S * kLmSlotBytes);
+    const std::vector<unsigned char> index = lm_index_bytes(mx->lm_index, B);
+    if ((rc = upload_slots(reinterpret_cast<HostScorer *const *>(mx->scorers), mx->S, index.data(), B, slots, slot_of,
+                           s)))
+      return rc;
+    io.lm_slots = slots; io.lm_slot_of = slot_of; io.lm_hist_stride = rep->max_order - 1;
+  }
   // (the host lengths only serve the hook scorers' handshake: the ARPA branch of the step reads the device copy)
   if ((rc = lm_batch_step(cfg, pl, sc, g_cache[device], device, nullptr, B, T, io, s))) return rc;
-  return launch_readout(sc, tokens, lens, n_results, scores, io.P * B, cfg->beam_size, T, s, io.lm_ab, B);
+  return launch_readout(sc, tokens, lens, n_results, scores, io.P * B, cfg->beam_size, T, s, io.lm_ab, B, io.lm_slots,
+                        io.lm_slot_of);
 }
 
 int ctcdec_decode_batch_lm_device_async(const ctcdec_config *cfg, void *scorer, const void *input, int dtype,
@@ -2076,6 +2340,16 @@ int ctcdec_decode_batch_lm_sweep_async(const ctcdec_config *cfg, void *scorer, c
   if (P < 1) return fail(CTCDEC_E_INVALID, "%d (alpha, beta) pairs: a sweep needs at least one", P);
   return lm_decode_async(cfg, scorer, input, dtype, seq_lens, B, T, alphas, betas, P, tokens, timesteps, scores, lens,
                          n_results, flags, log_probs_out, workspace, workspace_bytes, stream);
+}
+
+int ctcdec_decode_batch_lm_mixed_async(const ctcdec_config *cfg, void *const *scorers, int S, const int32_t *lm_index,
+                                       const void *input, int dtype, const int32_t *seq_lens, int B, int T,
+                                       int32_t *tokens, int32_t *timesteps, float *scores, int32_t *lens,
+                                       int32_t *n_results, int32_t *flags, float *log_probs_out, void *workspace,
+                                       size_t workspace_bytes, void *stream) {
+  const MixedCall mx{scorers, S, lm_index};
+  return lm_decode_async(cfg, nullptr, input, dtype, seq_lens, B, T, nullptr, nullptr, 0, tokens, timesteps, scores,
+                         lens, n_results, flags, log_probs_out, workspace, workspace_bytes, stream, &mx);
 }
 
 // Diagnostic: the read-out of [B, K] host rows, on the host (lm_rescore_batch through the scorer's hooks) or by the

@@ -31,9 +31,16 @@ Differences from the reference, all additive:
     device scorer on the GPU as well.
   * ``decode_sweep(x, alphas, betas)`` (device scorer): one batch under P (alpha, beta) pairs in one enqueue, results
     with a leading pair axis, each slice equal to ``decode`` after ``reset_params`` with that pair.
+  * ``decode_mixed(x, lm_index, decoders)`` (device scorer): one batch whose utterances need different language models
+    (per customer, domain or language) in one enqueue: utterance b is decoded with the model and weights of
+    ``decoders[lm_index[b]]``, bit for bit as that decoder's ``decode`` gives it; up to 16 models, all word-based or all
+    character-based, built for the same labels.
   * the [batch, beam, T] result tensors are PAGE-LOCKED CPU tensors (torch's caching host allocator, so a decode loop
     reuses the same blocks) up to CTCDECODE_B200_PIN_OUTPUT_BYTES per tensor (default 1 GiB), pageable beyond: a fresh
     pageable [256, 100, 1000] int32 pair costs page faults on every call, several times the decode itself.
+  * ``OnlineCTCBeamDecoder.decode`` / ``decode_logits`` take ``DecoderState``s of different device-scorer decoders
+    (``scorer_provider="device"``, same configuration and labels, up to 16 models) in one call, as the reference's
+    ``decode`` takes states of different decoders: each stream decodes with its own decoder's model and weights.
   * ``OnlineCTCBeamDecoder``: CUDA chunks (without a scorer, or with ``non_blocking=True``) are decoded in place on the
     current stream, raw logits go
     through ``decode_logits``, ``device_outputs=True`` leaves the results on the GPU, and ``committed_prefix`` reports
@@ -373,13 +380,87 @@ class CTCBeamDecoder(_Base):
         self.last_flags, self.last_n_results = flags.cpu(), n_results.cpu()
         return output.cpu(), scores.cpu(), timesteps.cpu(), out_seq_len.cpu()
 
+    def decode_mixed(self, x, lm_index, decoders, seq_lens=None, logits=False):
+        """Extension: decode one batch whose utterances need different language models in one enqueue
+        (ctcdec_decode_batch_lm_mixed_async): utterance b with the model and weights of decoders[lm_index[b]], each a
+        CTCBeamDecoder built with scorer_provider="device" (ARPA text or a KenLM binary; order, layout, alpha and beta may
+        differ), all word-based or all character-based and built for this decoder's labels.  At most
+        CTCDEC_LM_MIXED_MAX_MODELS (16) decoders.  This decoder's configuration (beam, cut, blank, log input) applies
+        to the whole batch.  x and seq_lens as in decode_sweep: [B, T, V] probabilities, CPU or CUDA, or with
+        logits=True raw float32 / float16 / bfloat16 CUDA logits.  Returns decode's four tensors and sets last_flags /
+        last_n_results; utterance b's results equal decoders[lm_index[b]].decode's (with this configuration) bit for
+        bit.  CPU input is uploaded and the call waits; CUDA input follows device_outputs / non_blocking as decode."""
+        from .scorer import ArpaScorer
+        decoders = list(decoders)
+        if not decoders:
+            raise ValueError("decoders must not be empty")
+        for i, d in enumerate(decoders):
+            if not isinstance(getattr(d, "_scorer", None), ArpaScorer):
+                raise ValueError('decoders[%d] has no language model with scorer_provider="device": a mixed decode '
+                                 "runs the device n-gram scorer" % i)
+            if list(d._labels) != self._labels:
+                raise ValueError("decoders[%d] was built for other labels than this decoder" % i)
+        if x.dim() != 3:
+            raise ValueError("x must be [batch, time, labels], got %s" % (tuple(x.shape),))
+        B, T, V = x.shape
+        if V != self._num_labels:
+            raise ValueError("x has %d labels, decoder was built with %d" % (V, self._num_labels))
+        lm_index = torch.as_tensor(lm_index).to(device="cpu", dtype=torch.int32).contiguous()
+        if lm_index.shape != (B,):
+            raise ValueError("lm_index must be [batch], got %s" % (tuple(lm_index.shape),))
+        dtype = -1
+        if logits:
+            dtypes = {torch.float32: 0, torch.float16: 1, torch.bfloat16: 2}
+            if not x.is_cuda or x.dtype not in dtypes:
+                raise ValueError("logits must be a float32, float16 or bfloat16 CUDA tensor")
+            dtype = dtypes[x.dtype]
+            x = x.contiguous()
+        host = not x.is_cuda
+        dev = x.device if not host else torch.device("cuda", self._device_index())
+        if dtype == -1:
+            x = x.to(device=dev, dtype=torch.float32).contiguous()
+        if seq_lens is not None:
+            seq_lens = seq_lens.to(device=dev, dtype=torch.int32).contiguous()
+        lib = _native.load()
+        cfg = _cfg(self)
+        K, S = self._beam_width, len(decoders)
+        scorers = (ctypes.c_void_p * S)(*[d._scorer.handle for d in decoders])
+        nbytes = ctypes.c_size_t(0)
+        _native.check(lib.ctcdec_lm_mixed_workspace_bytes(ctypes.byref(cfg), scorers, S, B, T, ctypes.byref(nbytes)))
+        if self._ws is None or self._ws.numel() < nbytes.value or self._ws.device != dev:
+            self._ws = None
+            self._ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        output = torch.empty(B, K, T, dtype=torch.int32, device=dev)
+        timesteps = torch.empty(B, K, T, dtype=torch.int32, device=dev)
+        scores = torch.empty(B, K, dtype=torch.float32, device=dev)
+        out_seq_len = torch.zeros(B, K, dtype=torch.int32, device=dev)
+        n_results = torch.zeros(B, dtype=torch.int32, device=dev)
+        flags = torch.zeros(B, dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            _native.check(lib.ctcdec_decode_batch_lm_mixed_async(
+                ctypes.byref(cfg), scorers, S, lm_index.data_ptr(), x.data_ptr(), dtype,
+                seq_lens.data_ptr() if seq_lens is not None else None, B, T, output.data_ptr(), timesteps.data_ptr(),
+                scores.data_ptr(), out_seq_len.data_ptr(), n_results.data_ptr(), flags.data_ptr(), None,
+                self._ws.data_ptr(), self._ws.numel(), stream))
+        self.last_flags, self.last_n_results = flags, n_results
+        if self._device_outputs and not host:
+            if not self._non_blocking:
+                torch.cuda.current_stream(dev).synchronize()
+                self._check_flags(flags)
+            return output, scores, timesteps, out_seq_len
+        torch.cuda.current_stream(dev).synchronize()
+        self._check_flags(flags)
+        self.last_flags, self.last_n_results = flags.cpu(), n_results.cpu()
+        return output.cpu(), scores.cpu(), timesteps.cpu(), out_seq_len.cpu()
+
     @staticmethod
     def _check_flags(flags):
         bad = (flags & _native.FLAG_ERR_ARENA).nonzero()
         if bad.numel():
-            p, b = (int(v) for v in bad[0])
-            raise _native.NativeError("pair %d, utterance %d: the beam kernel reported an internal error; results are "
-                                      "not valid" % (p, b))
+            where = "utterance %d" % int(bad[0][0]) if flags.dim() == 1 else \
+                "pair %d, utterance %d" % tuple(int(v) for v in bad[0])
+            raise _native.NativeError("%s: the beam kernel reported an internal error; results are not valid" % where)
 
 
 class OnlineCTCBeamDecoder(_Base):
@@ -503,7 +584,12 @@ class OnlineCTCBeamDecoder(_Base):
         K = self._beam_width
         cfg = _cfg(self)
         nbytes = ctypes.c_size_t(0)
-        _native.check(lib.ctcdec_stream_workspace_bytes(ctypes.byref(cfg), B, T, ctypes.byref(nbytes)))
+        handles = (ctypes.c_void_p * B)(*[s.state for s in states])
+        # (states of several device-scorer decoders need room for their LM slots as well)
+        if B:
+            _native.check(lib.ctcdec_stream_states_workspace_bytes(handles, B, T, ctypes.byref(nbytes)))
+        else:
+            _native.check(lib.ctcdec_stream_workspace_bytes(ctypes.byref(cfg), B, T, ctypes.byref(nbytes)))
         if self._ws is None or self._ws.numel() < nbytes.value or self._ws.device != dev:
             self._ws = None
             self._ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
@@ -513,7 +599,6 @@ class OnlineCTCBeamDecoder(_Base):
         out_seq_len = torch.zeros(B, K, dtype=torch.int32, device=dev)
         n_results = torch.zeros(B, dtype=torch.int32, device=dev)
         flags = torch.zeros(B, dtype=torch.int32, device=dev)
-        handles = (ctypes.c_void_p * B)(*[s.state for s in states])
         eos_arr = (ctypes.c_uint8 * B)(*[1 if e else 0 for e in eos])
         with torch.cuda.device(dev):
             stream = torch.cuda.current_stream(dev).cuda_stream

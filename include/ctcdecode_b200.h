@@ -322,6 +322,43 @@ int ctcdec_decode_batch_lm_sweep_async(const ctcdec_config *cfg, void *scorer, c
                                        int32_t *lens, int32_t *n_results, int32_t *flags, float *log_probs_out,
                                        void *workspace, size_t workspace_bytes, void *stream);
 
+/* The most language models one ctcdec_decode_batch_lm_mixed_async call takes: their LM slots (model tables, dictionary,
+ * order and weights) travel in the parameters of one kernel launch. */
+#define CTCDEC_LM_MIXED_MAX_MODELS 16
+
+/* Bytes of device scratch ctcdec_decode_batch_lm_mixed_async needs for S scorers over a [B, T, V] batch.  When all S
+ * pointers are one scorer, exactly ctcdec_lm_workspace_bytes(cfg, scorers[0], B, T).  Otherwise
+ * ctcdec_lm_workspace_bytes(cfg, m, B, T) for the scorer m of the largest order (the per-node LM histories take the
+ * largest order - 1 ids per node), less its 256 bytes of alignment slack, plus the slot table (256 bytes per scorer,
+ * 256-byte aligned), the utterances' slot indices (B bytes, 256-byte aligned) and the 256 bytes of slack.  The refusals
+ * of ctcdec_decode_batch_lm_mixed_async's checks of scorers and S, no device needed. */
+int ctcdec_lm_mixed_workspace_bytes(const ctcdec_config *cfg, void *const *scorers, int S, int B, int T, size_t *bytes);
+
+/* Extension: decode a batch whose utterances need different language models, in one enqueue.  Utterance b is decoded
+ * with the model and weights of scorers[lm_index[b]]: every output of it, flags included, is bit for bit what
+ * ctcdec_decode_batch_lm_device_async with that scorer gives for it -- against the sub-batch of that scorer's utterances
+ * whenever both calls get the same beam-kernel block size, which holds up to 264 utterances; above that the two block
+ * sizes may order comparator-equal rows (CTCDEC_FLAG_TIE_FINAL) differently.  Each scorer's alpha and beta are read
+ * when the call is made.  Every beam CTA finds its model through its LM slot; the read-out rescores each row with its
+ * utterance's model, front end and weights.  A call whose scorers are all one object is
+ * ctcdec_decode_batch_lm_device_async.
+ *   scorers [S]: scorers from ctcdec_scorer_create_arpa (ARPA text or any KenLM binary it takes; layout, order and
+ *              weights may differ), 1 <= S <= CTCDEC_LM_MIXED_MAX_MODELS, all built for the decoder's labels (string
+ *              for string) and all word-based or all character-based.
+ *   lm_index   HOST int32 [B], each in [0, S): checked on the host.
+ *   Everything else as ctcdec_decode_batch_lm_device_async: seq_lens a DEVICE int32 [B] buffer or NULL, device outputs,
+ *              no waiting, capturable into a CUDA graph after one decode with these scorers outside the capture (the
+ *              slots and indices travel in kernel launch parameters, so a graph replays the models and weights it
+ *              captured).  Workspace: ctcdec_lm_mixed_workspace_bytes.
+ * Refused: NULL scorers, S < 1 or S > CTCDEC_LM_MIXED_MAX_MODELS, NULL lm_index (B > 0) or an index outside [0, S), or
+ * scorers built for different labels: CTCDEC_E_INVALID; a hook scorer beside any other scorer, or word-based beside
+ * character-based models: CTCDEC_E_UNSUPPORTED. */
+int ctcdec_decode_batch_lm_mixed_async(const ctcdec_config *cfg, void *const *scorers, int S, const int32_t *lm_index,
+                                       const void *input, int dtype, const int32_t *seq_lens, int B, int T,
+                                       int32_t *tokens, int32_t *timesteps, float *scores, int32_t *lens,
+                                       int32_t *n_results, int32_t *flags, float *log_probs_out, void *workspace,
+                                       size_t workspace_bytes, void *stream);
+
 /* ---- streaming (OnlineCTCBeamDecoder) ------------------------------------------------------------- */
 
 /* Replaces: paddle_get_decoder_state (binding.cpp:246-261).  The state (beam + trie + absolute frame
@@ -343,7 +380,14 @@ int ctcdec_state_frames(const void *state, int *frames);
  * probs [B, T, V] and seq_lens are HOST buffers holding the next chunk of every stream; states[b] is
  * advanced by min(seq_lens[b], T) frames; for streams with is_eos[b] != 0 the current beams are written
  * to tokens/timesteps [B, beam, out_T] (rows of other streams untouched), scores/lens [B, beam].
- * out_T must be >= the longest prefix (the number of frames consumed is always enough). */
+ * out_T must be >= the longest prefix (the number of frames consumed is always enough).
+ * The states of one call share the decoder configuration and the device.  Their scorers are one object (or none), or,
+ * as the reference's per-state Scorer allows, different scorers from ctcdec_scorer_create_arpa -- at most
+ * CTCDEC_LM_MIXED_MAX_MODELS of them, all word-based or all character-based, built for the same labels: each stream
+ * then decodes with its own scorer's model, and its eos read-out uses that scorer's alpha and beta as they are when the
+ * call is made.  Refused: a different configuration or device, states with a scorer beside states without one, a hook
+ * scorer beside another scorer, word-based beside character-based models, more than CTCDEC_LM_MIXED_MAX_MODELS
+ * scorers (CTCDEC_E_UNSUPPORTED); scorers built for different labels (CTCDEC_E_INVALID). */
 int ctcdec_decode_stream_host(const float *probs, const int32_t *seq_lens, int B, int T, void *const *states,
                               const uint8_t *is_eos, int32_t *tokens, int32_t *timesteps, int out_T, float *scores,
                               int32_t *lens, int32_t *n_results, int32_t *flags);
@@ -351,6 +395,10 @@ int ctcdec_decode_stream_host(const float *probs, const int32_t *seq_lens, int B
 /* Bytes of device scratch one ctcdec_decode_stream_device call of B streams and T frames needs (the pruned rows of
  * the chunk and the per-call tables of stream pointers). */
 int ctcdec_stream_workspace_bytes(const ctcdec_config *cfg, int B, int T, size_t *bytes);
+/* The same for the B states of a call (B >= 1, checked as ctcdec_decode_stream_device checks them): exactly
+ * ctcdec_stream_workspace_bytes when their scorers are one object (or none); for states of S > 1 different scorers
+ * that plus their LM slots, al256(B) + al256(256 x S) bytes (al256: rounded up to a multiple of 256). */
+int ctcdec_stream_states_workspace_bytes(void *const *states, int B, int T, size_t *bytes);
 
 /* ctcdec_decode_stream_host with the chunk and the results on the DEVICE, enqueued on `stream` (a cudaStream_t of the
  * states' device, which must be the current device).  Extension: the reference decodes CPU tensors only.
