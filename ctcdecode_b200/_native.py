@@ -92,6 +92,8 @@ _SIGNATURES = {
                                                    _vp, _vp, ctypes.c_size_t, _vp]),
     "ctcdec_stream_committed_device": (ctypes.c_int, [ctypes.POINTER(_vp), ctypes.c_int, _vp, _vp, _vp, _vp,
                                                       ctypes.c_int, _vp]),
+    "ctcdec_stream_compact": (ctypes.c_int, [ctypes.POINTER(_vp), ctypes.c_int, _vp, _vp]),
+    "ctcdec_state_device_bytes": (ctypes.c_int, [_vp, ctypes.POINTER(ctypes.c_size_t)]),
     "ctcdec_profile_enable": (ctypes.c_int, [ctypes.c_int]),
     "ctcdec_profile_read": (ctypes.c_int, [ctypes.POINTER(ctypes.c_float)]),
     "ctcdec_profile_region_cycles": (ctypes.c_int, [_vp]),

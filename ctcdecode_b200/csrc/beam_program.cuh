@@ -2096,11 +2096,9 @@ CTC_FN void finalize_cta_run(const BeamParams &p, const int b, unsigned char *sm
 // ======================================================================================================
 constexpr int kCommitCp = 256;  // checkpoints of the write-out per round
 CTC_HD size_t committed_smem_bytes(int K) { return (size_t)K * 3 * 4 + (size_t)kCommitCp * 4 + 64; }
-// since: positions already read out (the previous call's result); outside [0, LCA depth] it is taken as 0.
-// Writes *committed = LCA depth and columns [0, min(depth - since, cap)) of out_tok / out_ts (positions since..).
+// Steps (a) and (b): returns the LCA depth D; with M > 0 the LCA's node id is left in ((int *)smem)[K] (s_hi[0]).
 template <int NT>
-CTC_FN void committed_cta_run(const Node *nodes, const int *st, int K, int since, int *committed, int *out_tok,
-                              int *out_ts, int cap, unsigned char *smem) {
+CTC_FN int members_lca(const Node *nodes, const int *st, int K, unsigned char *smem) {
   const int M = st[0];
   const int *s = st + kStateHeader;
   int *s_cur = (int *)smem;       // [K] each member's ancestor at the current aligned depth
@@ -2178,6 +2176,19 @@ CTC_FN void committed_cta_run(const Node *nodes, const int *st, int K, int since
     --D;
     CTC_BARRIER();
   }
+  return D;
+}
+
+// since: positions already read out (the previous call's result); outside [0, LCA depth] it is taken as 0.
+// Writes *committed = LCA depth and columns [0, min(depth - since, cap)) of out_tok / out_ts (positions since..).
+template <int NT>
+CTC_FN void committed_cta_run(const Node *nodes, const int *st, int K, int since, int *committed, int *out_tok,
+                              int *out_ts, int cap, unsigned char *smem) {
+  const int M = st[0];
+  const int D = members_lca<NT>(nodes, st, K, smem);
+  int *s_hi = (int *)smem + K;
+  int *s_cp = s_hi + 2 * K;
+  int *s_ctl = s_cp + kCommitCp;
   // (c) write positions [s0, min(D, s0 + cap)) of the path root -> LCA; node of depth d holds position d - 1
   const int s0 = (since >= 0 && since <= D) ? since : 0;
   CTC_PAR {

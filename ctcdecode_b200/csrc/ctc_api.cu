@@ -18,6 +18,7 @@
 
 #include "../../include/ctcdecode_b200.h"
 #include "beam_program.cuh"
+#include "compact_program.cuh"
 #include "plan.h"
 #include "lm_host.h"
 #include "prune_program.cuh"
@@ -60,6 +61,30 @@ __global__ void __launch_bounds__(NT) committed_kernel(const CommitArgs a) {
   const int i = (int)blockIdx.x, b = a.b0 + i;
   committed_cta_run<NT>(a.arena[i], a.state[i], a.K, a.since ? a.since[b] : 0, &a.committed[b],
                         a.tokens + (size_t)b * a.cap, a.timesteps + (size_t)b * a.cap, a.cap, smem);
+}
+
+// arena compaction of streaming states (compact_program.cuh): one CTA per stream, the stream's arrays in the launch
+// parameters, kCompactPerLaunch streams per launch
+constexpr int kCompactPerLaunch = 32;
+constexpr int kCompactNT = 256;
+struct CompactMarkArgs {
+  const Node *arena[kCompactPerLaunch];
+  const int *state[kCompactPerLaunch];
+  int *map[kCompactPerLaunch];
+  int K[kCompactPerLaunch], cap[kCompactPerLaunch];
+  int *kept;
+};
+__global__ void __launch_bounds__(kCompactNT) compact_mark_kernel(const CompactMarkArgs a) {
+  extern __shared__ __align__(128) unsigned char smem[];
+  const int i = (int)blockIdx.x;
+  compact_mark_cta_run<kCompactNT>(a.arena[i], a.state[i], a.K[i], a.cap[i], a.map[i], &a.kept[i], smem);
+}
+struct CompactGatherArgs {
+  CompactJob job[kCompactPerLaunch];
+};
+static_assert(sizeof(CompactGatherArgs) <= 4096, "the jobs must fit the kernel parameters");
+__global__ void __launch_bounds__(kCompactNT) compact_gather_kernel(const CompactGatherArgs a) {
+  compact_gather_cta_run<kCompactNT>(a.job[blockIdx.x]);
 }
 
 // The per-call tables of a streaming chunk (each stream's arena, state block, capacity, eos flag, scorer arrays and
@@ -607,6 +632,10 @@ struct StreamEvent {
   ~StreamEvent() { if (ev) cudaEventDestroy(ev); }
 };
 
+// Frames of room a streaming arena has beyond what its nodes need: at creation, and after a compaction (capacity
+// max(1 + beam x 256, kept + beam x 256) nodes)
+constexpr int kArenaSlackFrames = 256;
+
 // streaming state object
 struct StreamState {
   std::shared_ptr<StreamEvent> last;  // the last device-path call that used this state (or null)
@@ -616,6 +645,9 @@ struct StreamState {
   int arena_cap;
   int *state;
   int frames;
+  // node accounting: the arena holds at most node_base + beam x since nodes (node_base: nodes kept by the last
+  // compaction, 1 before any; since: frames consumed after it)
+  long long node_base = 1, since = 0;
   // scorer path (ctcdec_state_create_lm): the borrowed scorer (reference DecoderState::ext_scorer,
   // ctc_beam_search_decoder.cpp:31), per-node LM terms / dictionary states, the host mirror of the trie
   HostScorer *sc = nullptr;
@@ -1222,7 +1254,7 @@ static int state_create(const ctcdec_config *cfg, int device, bool lm, void **st
   if ((rc = use_device(device))) return rc;
   StreamState *st = new StreamState();
   st->cfg = *cfg; st->device = device; st->frames = 0; st->arena = nullptr; st->state = nullptr;
-  st->arena_cap = 1 + cfg->beam_size * 256;
+  st->arena_cap = 1 + cfg->beam_size * kArenaSlackFrames;
   if (cudaMalloc(&st->arena, (size_t)st->arena_cap * sizeof(Node)) != cudaSuccess ||
       cudaMalloc(&st->state, (size_t)state_ints(cfg->beam_size) * 4) != cudaSuccess) {
     if (st->arena) cudaFree(st->arena);
@@ -1368,20 +1400,21 @@ static int record_device_work(void *const *states, int B, cudaStream_t s) {
   return CTCDEC_OK;
 }
 
-// Grow each arena so that 1 + K * (frames consumed after this chunk) nodes fit.  Doubling keeps this to about
+// Grow each arena so that node_base + K * (frames since the last compaction, this chunk included) nodes fit: for a
+// state never compacted, 1 + K * (frames consumed after this chunk).  Doubling keeps this to about
 // log2(frames / 256) times per stream; the copy runs on s (after the stream's earlier work) and the host waits for
 // it before the old arrays are freed.
 static int grow_arenas(void *const *states, int B, const int *clen, cudaStream_t s) {
   for (int b = 0; b < B; ++b) {
     StreamState *sb = static_cast<StreamState *>(states[b]);
     const int K = sb->cfg.beam_size, V = sb->cfg.vocab_size;
-    const long long need = 1 + (long long)K * (sb->frames + clen[b]);
+    const long long need = sb->node_base + (long long)K * (sb->since + clen[b]);
     if (need <= sb->arena_cap) continue;
     long long cap = std::max<long long>(need, 2ll * sb->arena_cap);
     if (cap > 0x7fffffffll / 2) return fail(CTCDEC_E_UNSUPPORTED, "stream too long for the node arena");
     Node *na = nullptr;
     CU(cudaMalloc(&na, (size_t)cap * sizeof(Node)));
-    const long long used = std::min<long long>(sb->arena_cap, 1 + (long long)K * sb->frames);
+    const long long used = std::min<long long>(sb->arena_cap, sb->node_base + (long long)K * sb->since);
     CU(cudaMemcpyAsync(na, sb->arena, (size_t)used * sizeof(Node), cudaMemcpyDeviceToDevice, s));
     CU(cudaStreamSynchronize(s));
     CU(cudaFree(sb->arena));
@@ -1506,7 +1539,11 @@ static int stream_chunk_step(const ctcdec_config &cfg, Plan &pl, void *const *st
   } else if (T > 0 && (rc = launch_beam(bp, pl, B, s))) {
     return rc;
   }
-  for (int b = 0; b < B; ++b) static_cast<StreamState *>(states[b])->frames += clen[b];
+  for (int b = 0; b < B; ++b) {
+    StreamState *sb = static_cast<StreamState *>(states[b]);
+    sb->frames += clen[b];
+    sb->since += clen[b];
+  }
   if (any_eos && (rc = launch_finalize(bp, B, s))) return rc;
   return CTCDEC_OK;
 }
@@ -1717,6 +1754,135 @@ int ctcdec_stream_committed_device(void *const *states, int B, const int32_t *si
     CU(cudaGetLastError());
   }
   return record_device_work(states, B, s);
+}
+
+// Device bytes of one state's arrays of `cap` nodes: arena, and with a scorer the LM terms and histories, dictionary
+// states and a character-based model's rows.
+static size_t state_arena_bytes(const StreamState *st, long long cap) {
+  size_t n = (size_t)cap * sizeof(Node);
+  if (st->sc) n += (size_t)cap * (1 + st->lm_hist_n) * 4 + (size_t)cap * 4;
+  if (st->lm_row) n += (size_t)cap * st->cfg.vocab_size * 4;
+  return n;
+}
+
+int ctcdec_state_device_bytes(const void *state, size_t *bytes) {
+  if (!state || !bytes) return fail(CTCDEC_E_INVALID, "NULL argument");
+  const StreamState *st = static_cast<const StreamState *>(state);
+  *bytes = state_arena_bytes(st, st->arena_cap) + (size_t)state_ints(st->cfg.beam_size) * 4;
+  return CTCDEC_OK;
+}
+
+int ctcdec_stream_compact(void *const *states, int B, int64_t *nodes_kept, void *stream) {
+  if (B <= 0) return B == 0 ? CTCDEC_OK : fail(CTCDEC_E_INVALID, "negative batch");
+  if (!states) return fail(CTCDEC_E_INVALID, "states is NULL");
+  for (int b = 0; b < B; ++b) {
+    if (!states[b]) return fail(CTCDEC_E_INVALID, "states[%d] is NULL", b);
+    for (int a = 0; a < b; ++a)
+      if (states[a] == states[b]) return fail(CTCDEC_E_INVALID, "states[%d] and states[%d] are the same object", a, b);
+  }
+  StreamState *s0 = static_cast<StreamState *>(states[0]);
+  for (int b = 0; b < B; ++b) {
+    const StreamState *sb = static_cast<const StreamState *>(states[b]);
+    if (sb->device != s0->device) return fail(CTCDEC_E_UNSUPPORTED, "all states of one call must live on one device");
+    if (sb->sc && !sb->sc->ngram)
+      return fail(CTCDEC_E_UNSUPPORTED, "states[%d] has a hook scorer: the host's mirror of its trie is indexed by node "
+                  "id, so its arena cannot be compacted", b);
+  }
+  int rc = check_current_device(s0);
+  if (rc) return rc;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+  cudaStreamCaptureStatus capturing = cudaStreamCaptureStatusNone;
+  CU(cudaStreamIsCapturing(s, &capturing));
+  if (capturing != cudaStreamCaptureStatusNone)
+    return fail(CTCDEC_E_UNSUPPORTED, "ctcdec_stream_compact cannot be captured into a CUDA graph: it waits for the "
+                "device and allocates the compacted arrays");
+  size_t smem = 0, map_ints = 0;
+  for (int b = 0; b < B; ++b) {
+    const StreamState *sb = static_cast<const StreamState *>(states[b]);
+    smem = std::max(smem, compact_smem_bytes(sb->cfg.beam_size, kCompactNT));
+    map_ints += (size_t)sb->arena_cap;
+  }
+  if ((rc = raise_smem_limit<compact_mark_kernel>(smem, "compaction"))) return rc;
+  std::lock_guard<std::mutex> lock(g_mu[s0->device]);
+  if ((rc = wait_device_work(states, B, s))) return rc;
+  // scratch: every stream's id map (at most arena_cap nodes each), then the kept counts
+  int *scratch = nullptr;
+  CU(cudaMalloc(&scratch, (map_ints + B) * 4));
+  std::unique_ptr<int, cudaError_t (*)(void *)> scratch_owner(scratch, cudaFree);
+  int *const d_kept = scratch + map_ints;
+  std::vector<int *> maps(B);
+  size_t o = 0;
+  for (int b = 0; b < B; o += static_cast<StreamState *>(states[b])->arena_cap, ++b) maps[b] = scratch + o;
+  for (int b0 = 0; b0 < B; b0 += kCompactPerLaunch) {
+    CompactMarkArgs a;
+    memset(&a, 0, sizeof(a));
+    const int n = std::min(kCompactPerLaunch, B - b0);
+    for (int i = 0; i < n; ++i) {
+      const StreamState *sb = static_cast<const StreamState *>(states[b0 + i]);
+      a.arena[i] = sb->arena; a.state[i] = sb->state; a.map[i] = maps[b0 + i]; a.K[i] = sb->cfg.beam_size;
+      a.cap[i] = sb->arena_cap;
+    }
+    a.kept = d_kept + b0;
+    compact_mark_kernel<<<n, kCompactNT, smem, s>>>(a);
+    CU(cudaGetLastError());
+  }
+  std::vector<int> kept(B);
+  CU(cudaMemcpyAsync(kept.data(), d_kept, (size_t)B * 4, cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s));
+  // the compacted arrays; on a failure here nothing has changed yet
+  struct Fresh { Node *arena = nullptr; float *lm = nullptr, *row = nullptr; int *dst = nullptr; long long cap = 0; };
+  std::vector<Fresh> nw(B);
+  auto free_fresh = [&](bool which_new) {
+    for (int b = 0; b < B; ++b) {
+      StreamState *sb = static_cast<StreamState *>(states[b]);
+      if (which_new) { cudaFree(nw[b].arena); cudaFree(nw[b].lm); cudaFree(nw[b].dst); cudaFree(nw[b].row); }
+      else { cudaFree(sb->arena); cudaFree(sb->lm_arena); cudaFree(sb->dstate); cudaFree(sb->lm_row); }
+    }
+  };
+  for (int b = 0; b < B; ++b) {
+    const StreamState *sb = static_cast<const StreamState *>(states[b]);
+    const long long K = sb->cfg.beam_size;
+    Fresh &f = nw[b];
+    f.cap = std::max<long long>(1 + K * kArenaSlackFrames, kept[b] + K * kArenaSlackFrames);
+    bool ok = cudaMalloc(&f.arena, (size_t)f.cap * sizeof(Node)) == cudaSuccess;
+    if (ok && sb->sc)
+      ok = cudaMalloc(&f.lm, (size_t)f.cap * (1 + sb->lm_hist_n) * 4) == cudaSuccess &&
+           cudaMalloc(&f.dst, (size_t)f.cap * 4) == cudaSuccess;
+    if (ok && sb->lm_row) ok = cudaMalloc(&f.row, (size_t)f.cap * sb->cfg.vocab_size * 4) == cudaSuccess;
+    if (!ok) {
+      cudaGetLastError();
+      free_fresh(true);
+      return fail(CTCDEC_E_CUDA, "cudaMalloc failed for the compacted arrays of stream %d; the states are unchanged", b);
+    }
+  }
+  for (int b0 = 0; b0 < B; b0 += kCompactPerLaunch) {
+    CompactGatherArgs a;
+    memset(&a, 0, sizeof(a));
+    const int n = std::min(kCompactPerLaunch, B - b0);
+    for (int i = 0; i < n; ++i) {
+      const StreamState *sb = static_cast<const StreamState *>(states[b0 + i]);
+      const Fresh &f = nw[b0 + i];
+      CompactJob &j = a.job[i];
+      j.arena = sb->arena; j.arena_new = f.arena; j.state = sb->state; j.map = maps[b0 + i];
+      j.lm = sb->lm_arena; j.lm_new = f.lm; j.dst = sb->dstate; j.dst_new = f.dst; j.row = sb->lm_row; j.row_new = f.row;
+      j.K = sb->cfg.beam_size; j.cap = sb->arena_cap; j.cap_new = (int)f.cap; j.H = sb->lm_hist_n;
+      j.V = sb->cfg.vocab_size; j.kept = kept[b0 + i];
+    }
+    compact_gather_kernel<<<n, kCompactNT, 0, s>>>(a);
+    CU(cudaGetLastError());
+  }
+  if ((rc = record_device_work(states, B, s))) return rc;
+  CU(cudaStreamSynchronize(s));
+  free_fresh(false);
+  for (int b = 0; b < B; ++b) {
+    StreamState *sb = static_cast<StreamState *>(states[b]);
+    const Fresh &f = nw[b];
+    sb->arena = f.arena; sb->lm_arena = f.lm; sb->dstate = f.dst; sb->lm_row = f.row; sb->arena_cap = (int)f.cap;
+    sb->node_base = kept[b];
+    sb->since = 0;
+    if (nodes_kept) nodes_kept[b] = kept[b];
+  }
+  return CTCDEC_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -665,6 +665,28 @@ class OnlineCTCBeamDecoder(_Base):
             return tok, ts, n_new, committed
         return tok.cpu(), ts.cpu(), n_new.cpu(), committed.cpu()
 
+    def compact(self, states):
+        """Extension: frees the parts of each stream's trie that no later call can read (ctcdec_stream_compact).  A
+        stream's node arena otherwise grows by up to beam_width nodes per frame for as long as the stream lives; after
+        this call it holds only the paths from the root to the current beam members, and every later result of the
+        stream is bit for bit what it would have been without the call.  A server calls it every so many chunks, like
+        committed_prefix.  Waits for the device.  States of a hook scorer (scorer_provider other than "device") are
+        refused.  Returns the nodes each state holds now: int64 CPU tensor [B]."""
+        lib = _native.load()
+        B = len(states)
+        kept = torch.zeros(B, dtype=torch.int64)
+        if B == 0:
+            return kept
+        devs = {s.device for s in states}
+        if len(devs) != 1:
+            raise ValueError("all states must live on one device, got %s" % sorted(devs))
+        dev = torch.device("cuda", devs.pop())
+        handles = (ctypes.c_void_p * B)(*[s.state for s in states])
+        with torch.cuda.device(dev):
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            _native.check(lib.ctcdec_stream_compact(handles, B, kept.data_ptr(), stream))
+        return kept
+
     def reset_state(state):  # noqa: N805 -- signature kept from the reference (:249), which lacks `self`
         state.release()
 
@@ -682,6 +704,12 @@ class DecoderState(object):
         self.device = decoder._device_index()
         _native.check(lib.ctcdec_state_create_lm(ctypes.byref(cfg), scorer, self.device, ctypes.byref(handle)))
         self.state = handle.value
+
+    def device_bytes(self):
+        """Extension: the device memory this state holds (node arena, state block, scorer arrays), in bytes."""
+        n = ctypes.c_size_t(0)
+        _native.check(_native.load().ctcdec_state_device_bytes(self.state, ctypes.byref(n)))
+        return n.value
 
     def release(self):
         if getattr(self, "state", None):

@@ -442,6 +442,25 @@ int ctcdec_decode_stream_device(const void *probs, int dtype, const int32_t *seq
 int ctcdec_stream_committed_device(void *const *states, int B, const int32_t *since, int32_t *committed,
                                    int32_t *tokens, int32_t *timesteps, int cap, void *stream);
 
+/* Extension: compaction of streaming states.  A state's node arena only grows while it decodes (up to beam nodes per
+ * frame); everything a later chunk, eos read-out or ctcdec_stream_committed_device can read lies on the paths from
+ * the root to the current beam members.  This call keeps exactly those nodes, renumbered in their old order (the
+ * root stays 0, a parent below its children), with their LM terms, histories, dictionary states and rows, rewrites the
+ * node ids in each state block and frees the old arrays.  Every later output of a compacted stream equals, bit for
+ * bit, that of the same stream never compacted (DESIGN.md, "Streaming on the device").
+ *   nodes_kept  host int64 [B] or NULL: the nodes each state holds now.
+ * Capacity after the call: max(1 + beam x 256, kept + beam x 256) nodes; decoding grows it again as it needs, by the
+ * nodes kept plus beam x frames consumed since.
+ * The states may come from different configurations and scorers but must live on one device, the current one.
+ * Ordered after the states' pending device-path work on `stream`; the call waits for the device twice (to size the
+ * new arrays, and before freeing the old ones) and returns when it is done.  Refused before anything is enqueued:
+ * NULL or duplicate states (CTCDEC_E_INVALID), states with a hook scorer (CTCDEC_E_UNSUPPORTED: the host mirror of
+ * their trie is indexed by node id), states of several devices, and a stream being captured into a CUDA graph
+ * (CTCDEC_E_UNSUPPORTED).  An allocation failure leaves every state as it was. */
+int ctcdec_stream_compact(void *const *states, int B, int64_t *nodes_kept, void *stream);
+/* Extension: the device memory a streaming state holds: its node arena, state block and scorer arrays. */
+int ctcdec_state_device_bytes(const void *state, size_t *bytes);
+
 /* ---- measurement hook (bench.py) --------------------------------------------------------------------
  * With profiling enabled on the calling thread, ctcdec_decode_batch_device records CUDA events on its stream
  * around each of its kernels; ctcdec_profile_read waits for the last decode of this thread and returns
